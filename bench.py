@@ -1,6 +1,6 @@
-"""bench.py -- end-to-end tracked frames/s (detect + NMS + associate) of the B200-native path, and the CPU reference arm.
+"""bench.py -- end-to-end tracked frames/s (detect + NMS + associate) of the H100-native path, and the CPU reference arm.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload pipeline|tracker]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload pipeline|tracker] [--dump-outputs DIR]
 
 Default workload "pipeline" (bench_pipeline.py) = the BASELINE.json metric: YOLOv7-w6 1280 x 1280, batch 8 -> decode + NMS ->
 ByteTrack, one uint8 frame per sequence per step; its JSON line also carries BASELINE configs C1 / C3 / C4 / C5, C4 end to end with the
@@ -12,8 +12,11 @@ collective; one tiny all-gather of per-sequence birth counts gives the global tr
 Printed JSON (rank 0, one line):
   value         frames/s with the inputs already resident in HBM
   e2e           frames/s through the public API with HOST buffers: pinned H2D of the step's inputs + D2H of the tracks, every step
-  roofline      the dominant kernel against MEASURED_PEAKS.json
+  roofline      the dominant kernel against MEASURED_PEAKS.json (else the H100 SXM data sheet)
   cpu_baseline  the reference's CPU path on a bounded sample (N = 1 only)
+
+--dump-outputs DIR writes what the timed path returned in its last timed step (track rows, track counters) as DIR/<name>.npy
+(float64): the inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -55,7 +58,22 @@ def _peaks():
             p = json.load(f)
         return float(p["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "H100 SXM data sheet"
+
+
+def dump_outputs(out_dir, tracks, counters):
+    """--dump-outputs: the track rows (sequence, row, column) and the per-sequence track counters of one step as out_dir/<name>.npy,
+    float64 (integer counters are exact in it).  Rows past a sequence's output count are not results: they are written as zeros."""
+    if not out_dir:
+        return
+    from b200track import _lib as L
+    tracks = np.array(tracks, dtype=np.float64)
+    counters = np.array(counters, dtype=np.float64)
+    for s, n in enumerate(counters[:, L.STAT_NOUT].astype(np.int64)):
+        tracks[s, n:] = 0.0
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "tracks.npy"), tracks)
+    np.save(os.path.join(out_dir, "track_counters.npy"), counters)
 
 
 class ClockSampler(threading.Thread):
@@ -122,16 +140,6 @@ class ClockSampler(threading.Thread):
                 "reasons": sorted(self.reasons), "samples": self.n, "source": self.source}
 
 
-def _tracker_traffic(n_seq):
-    """DRAM bytes per launch of track_step_kernel from the committed ncu --set full capture (taken at 4 sequences)."""
-    try:
-        names = sorted(f for f in os.listdir(os.path.join(ROOT, "profiles")) if f.endswith("_track_step_traffic.json"))
-        tj = json.load(open(os.path.join(ROOT, "profiles", names[-1])))
-        return (tj["dram_bytes_read"] + tj["dram_bytes_write"]) if n_seq == 4 else None
-    except Exception:
-        return None
-
-
 def algorithmic_bytes(stat_rows, esize):
     """SURVEY.md section 8(d) per-unit figures x the units of this launch: predict 144 values/track
     (72 read + 72 written), update 148 values/matched track, IoU + LAP one write + one read of every
@@ -147,8 +155,8 @@ def algorithmic_bytes(stat_rows, esize):
 
 
 def run_reference_arm(args, rank, world):
-    """Reference arm: the reference's own CPU implementation of the path -- the reference is pure
-    Python and cannot travel to the GPU box, so this is the oracle port of it (oracle/trackers.py,
+    """Reference arm: the reference's own CPU implementation of the path -- the reference's tracker
+    is pure Python, so this is the oracle port of it (oracle/trackers.py,
     checked bit-for-bit against the reference in tests/golden), single thread like the reference."""
     if rank != 0:
         return
@@ -194,6 +202,8 @@ def parse_args():
     ap.add_argument("--no-sub", action="store_true", help="pipeline: skip config.sub_benchmarks (C3 / C4 / C5)")
     ap.add_argument("--quick-sub", action="store_true", help="pipeline: shorter sub-benchmarks")
     ap.add_argument("--no-cpu", action="store_true", help="pipeline: skip the cpu_baseline leg")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float64) for comparing two builds")
     return ap.parse_args()
 
 
@@ -209,8 +219,6 @@ def main():
     world = int(os.environ.get("WORLD_SIZE", "1"))
 
     if args.impl == "reference":
-        if args.steps > 200:
-            args.steps = 200
         run_reference_arm(args, rank, world)
         return
 
@@ -241,7 +249,7 @@ def main():
         eng.set_out_rows(512)
         return eng
 
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)      # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)      # > the 50 MB L2 of an H100
 
     # ---------------- device-resident arm: detections already in HBM
     eng = fresh_engine()
@@ -269,6 +277,9 @@ def main():
     torch.cuda.synchronize()
     t_wall = time.perf_counter() - t_wall0
     launches = lib.b2t_launch_count() - launches0
+    if rank == 0:
+        last = d_stat[STREAM_WARM + W + K - 1].cpu().numpy()
+        dump_outputs(args.dump_outputs, d_out.cpu().numpy(), last[:, :L.STAT_PHASE0])
     dev_ms = np.array([a.elapsed_time(b) for a, b in ev])
     step_ms = float(dev_ms.sum())
     stat_host = d_stat[STREAM_WARM + W:].cpu().numpy()
@@ -301,10 +312,10 @@ def main():
         nb = len(res_b[s])
         assert np.array_equal(ids_a[s, :nb], res_b[s][:, 0]), "device-resident and host-buffer arms disagree"
 
-    # ---------------- scale-out over sequences on one GPU: one CTA per sequence, 148 SMs
+    # ---------------- scale-out over sequences on one GPU: one CTA per sequence, one per SM of an H100 SXM
     sweep = {}
     if rank == 0 and world == 1:
-        for S2 in (148,):
+        for S2 in (132,):
             engs = TrackEngine(args.tracker, n_seq=S2, dtype=args.dtype, cap=1024, dmax=dmax, device=dev)
             dd = torch.from_numpy(np.ascontiguousarray(np.tile(dets_all[:STREAM_WARM + 40], (1, (S2 + S - 1) // S, 1, 1))[:, :S2])).to(dev)
             dc = torch.from_numpy(np.ascontiguousarray(np.tile(cnt_all[:STREAM_WARM + 40], (1, (S2 + S - 1) // S))[:, :S2])).to(dev)
@@ -366,7 +377,7 @@ def main():
                     "d2h_bytes_per_step": int(eng2.d2h_bytes_per_step), "ms_per_step": e2e_ms_max / K},
             "gpu_launches": int(launches),
             "roofline": {"bound": "hbm", "kernel": "track_step_kernel<%s>" % ("double" if esize == 8 else "float"),
-                         "achieved": achieved, "peak": hbm, "unit": "GB/s", "frac": achieved / hbm, "traffic": _tracker_traffic(S),
+                         "achieved": achieved, "peak": hbm, "unit": "GB/s", "frac": achieved / hbm,
                          "peak_source": how, "algorithmic_bytes_per_launch": algo_bytes, "kernel_us": kern_us,
                          "note": "latency-bound: one CTA per sequence, %d CTAs per launch (SURVEY 8d: ~1 MB/frame/sequence)" % S},
             "cpu_baseline": cpu,

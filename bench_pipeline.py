@@ -3,7 +3,7 @@
 One "step" = one 1280 x 1280 frame for each of the B sequences a rank owns (BASELINE config C2 + C3: YOLOv7-w6, batch 8,
 detect + NMS, then ByteTrack on the <= 300 detections per frame):
     uint8 BGR frames (as cv2.imread / tracker_dataloader.py:64-79 produce them)
-      -> letterbox + BGR->RGB + /255 + ReOrg + NHWC fp16 (one kernel) -> 96 tcgen05 conv launches (107 convs)
+      -> letterbox + BGR->RGB + /255 + ReOrg + NHWC fp16 (one kernel) -> 96 wgmma conv launches (107 convs)
       -> Detect decode fused with NMS (+ scale_coords / clip / round)                                             [CUDA graphs]
       -> fused ByteTrack step (one CTA per sequence) on the device-resident detections.
 value : the frames already resident in HBM (uint8), tracks read back.
@@ -43,23 +43,6 @@ def make_frames(batch, size, seed):
     return [np.ascontiguousarray(np.roll(base, (2 * k, k), axis=(1, 2))) for k in range(POOL)]
 
 
-def conv_traffic(n_conv):
-    """DRAM bytes of the conv launches of one step from the newest committed ``ncu --set full`` capture of this command
-    (profiles/*_conv_traffic.json, written by tools/summarize_profiles.py).  Returns (bytes per step, source, partial)."""
-    try:
-        pdir = os.path.join(ROOT, "profiles")
-        for cand in sorted((f for f in os.listdir(pdir) if f.endswith("_conv_traffic.json")), reverse=True):
-            tj = json.load(open(os.path.join(pdir, cand)))
-            total = tj["dram_bytes_read"] + tj["dram_bytes_write"]
-            if tj.get("launches") == n_conv:
-                return total, "profiles/" + cand, None
-            return None, None, {"launches": tj.get("launches"), "dram_bytes": total,
-                                "algorithmic_bytes": tj.get("algorithmic_bytes_same_launches"), "source": "profiles/" + cand}
-    except Exception:
-        pass
-    return None, None, None
-
-
 def run_reference(args, rank, world):
     """--impl reference: the reference's own CPU path (bench_reference.py), one frame per step, rank 0 only."""
     if rank != 0:
@@ -69,14 +52,14 @@ def run_reference(args, rank, world):
     from b200track.w6 import calibrated_state_dict
     sd = calibrated_state_dict(0, args.img, "cuda" if torch.cuda.is_available() else "cpu")
     sd = {k: v.cpu() for k, v in sd.items()}
-    n = max(1, min(args.steps, 30))                              # ~2 s per frame on 32 cores: bounded to about a minute
+    n = max(1, args.steps)
     w = max(1, min(args.warmup, 2))
     r = BR.run_cpu_arm(sd, args.img, n, w)
     fps = r["value"]
     line = {"impl": "reference", "metric": METRIC, "value": fps, "unit": "frames/s", "n_gpus": world, "steps": n, "warmup": w,
             "ms_per_step": 1e3 / fps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": _workload(args) + " [CPU arm: one frame per step, batch 1 like tracker/track.py:138-179]",
-                       "requested_steps": args.steps, "ms_per_frame": r["ms_per_frame"]},
+                       "ms_per_frame": r["ms_per_frame"]},
             "cpu_baseline": {"value": fps, "unit": "frames/s", "cores": r["cores"], "kind": r["kind"], "sample": r["sample"]},
             "e2e": {"value": fps, "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     print(json.dumps(line))
@@ -92,7 +75,7 @@ def run(args):
         return run_reference(args, rank, world)
 
     import torch.distributed as dist
-    from bench import ClockSampler
+    from bench import ClockSampler, dump_outputs
     from b200track import _lib as L
     from b200track.detector import DetectorW6
     from b200track.engine import TrackEngine
@@ -106,8 +89,8 @@ def run(args):
         dist.init_process_group("nccl", device_id=dev)
     lib = L.load()
     peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-    tf_peak = float(peaks.get("bf16_tflops_sustained", 1400.0))
-    hbm_gbs = float(peaks.get("hbm_gbs", 6650.0))
+    tf_peak = float(peaks.get("bf16_tflops_sustained", 989.0))      # H100 SXM data sheet, dense fp16 / bf16
+    hbm_gbs = float(peaks.get("hbm_gbs", 3350.0))
     sd = calibrated_state_dict(0, args.img, dev)
     det = DetectorW6(sd, batch=B, img_size=args.img, device=dev, use_graph=True)
     det.set_source_frames((args.img, args.img))
@@ -137,10 +120,10 @@ def run(args):
         e0.record(pipe.s_copy)
         for k in range(steps):
             pipe.step(dev_frames[k % POOL])
-        pipe.flush()
+        res = pipe.flush()
         e1.record(pipe.s_trk)
         torch.cuda.synchronize()
-        return e0.elapsed_time(e1)
+        return e0.elapsed_time(e1), res
 
     def timed_e2e(steps):
         torch.cuda.synchronize()
@@ -154,17 +137,17 @@ def run(args):
         return 1e3 * (time.perf_counter() - t0), res
 
     sampler = ClockSampler(local_rank); sampler.start()
-    torch.cuda.profiler.start()                                  # ncu --profile-from-start off: only the timed region
     l0 = lib.b2t_launch_count()
-    dev_ms = timed_device(K)                                     # ---- the K timed steps: frames resident in HBM
+    dev_ms, (d_out, d_stat) = timed_device(K)                    # ---- the K timed steps: frames resident in HBM
     tracker_launches = lib.b2t_launch_count() - l0
+    if rank == 0:       # the tracks of the last timed step and their counters (the phase cycle counters after them are timings)
+        dump_outputs(args.dump_outputs, d_out.numpy(), d_stat.numpy()[:, :L.STAT_PHASE0])
     e2e_ms, (h_out, h_stat) = timed_e2e(K)                       # ---- the K timed steps through the public API with HOST frames
-    torch.cuda.profiler.stop()
     clocks = sampler.summary()
     stat = pipe.t_stat.cpu().numpy()
     assert int(stat[:, L.STAT_ERR].max()) == 0
     # ---- repeats: the timed region is ~0.4 s; two more runs of the same K steps show the run-to-run spread
-    rep_dev = [dev_ms] + [timed_device(K) for _ in range(2)]
+    rep_dev = [dev_ms] + [timed_device(K)[0] for _ in range(2)]
     rep_e2e = [e2e_ms] + [timed_e2e(K)[0] for _ in range(2)]
     # phase cycles of the last track_step_kernel launch under the pipeline's own load (stat words 16..28, SM clocks; mean over sequences)
     phase_names = ["P0 dets", "P1 lists", "P2 predict", "P3 boxes", "P4 csr1", "P5 lap1", "P6 apply1", "P7 assoc2", "P8 assoc3", "P9 births",
@@ -262,7 +245,6 @@ def run(args):
         value = frames / (float(t[0]) / 1e3)
         e2e = frames / (float(t[1]) / 1e3)
         conv_tflops = det.flops / (conv_ms * 1e-3) / 1e12
-        traffic, traffic_src, traffic_partial = conv_traffic(n_conv)
         cpu = None
         if world == 1 and not args.no_cpu:
             import bench_reference as BR
@@ -292,9 +274,8 @@ def run(args):
                     "d2h_bytes_per_step": int(h_out.numel() * 8 + h_stat.numel() * 4), "ms_per_step": float(t[1]) / K},
             "gpu_launches": int(K * n_graph_kernels + tracker_launches),
             "roofline": {"bound": "tensor", "kernel": "conv_bias_act_kernel (%d launches per step: the 107 convs of the graph, ELAN 1x1 pairs stacked)" % n_conv,
-                         "achieved": conv_tflops, "peak": tf_peak, "unit": "TFLOP/s", "frac": conv_tflops / tf_peak, "traffic": traffic,
-                         "traffic_unit": "bytes per step (all conv launches)", "traffic_source": traffic_src, "traffic_partial": traffic_partial,
-                         "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (a kernel timed inside a long step)" if peaks else "fallback 1400 (sustained)",
+                         "achieved": conv_tflops, "peak": tf_peak, "unit": "TFLOP/s", "frac": conv_tflops / tf_peak,
+                         "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (a kernel timed inside a long step)" if peaks else "H100 SXM data sheet (989, dense)",
                          "algorithmic_flops_per_step": det.flops, "conv_ms_per_step": conv_ms,
                          "note": "algorithmic 2 x MAC of the 107 convs (SURVEY 8d: 359.7 GFLOP/img; the 255-channel heads are counted at 255) x batch / "
                                  "CUDA-event time of the conv launches replayed back to back as one graph"},

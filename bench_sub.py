@@ -1,5 +1,5 @@
 """Sub-benchmarks of the default bench line (``config.sub_benchmarks``): the BASELINE.json configurations that are not the
-headline, measured in the same run on the same GPU so that the driver's one command records them.
+headline, measured in the same run on the same GPU so that one command records them.
 
   C1  the reference's CPU-runnable plumbing case: YOLOv7-tiny on one 1280 x 1280 frame + ByteTrack update on 50 detections.
   C3  ByteTrack full loop, ~300 detections / frame, ~250 live tracks, 4 sequences per launch, detections resident in HBM,
@@ -201,7 +201,7 @@ def gmc_estimation(torch, dev, hbm_gbs, n_seq=8, size=1280, steps=40, cpu_frames
 
 def reid_features(torch, dev, n_crops=256, steps=20, cpu_crops=16):
     """SURVEY 8f row 3: the ReID extractor (tracker/reid_models/deepsort_reid.py:63-153) on n_crops windows of one frame per call --
-    crop / resize / normalise, 20 tcgen05 convolutions, batch-statistics BatchNorm, pooling -- with the reference's own Net timed on
+    crop / resize / normalise, 20 wgmma convolutions, batch-statistics BatchNorm, pooling -- with the reference's own Net timed on
     the host cores beside it (seeded weights: the 46 MB checkpoint does not travel)."""
     import time
     from b200track.reid import ReidExtractor

@@ -1,8 +1,8 @@
-/* b200track.h -- C ABI of libb200track.so (B200 / sm_100a).
+/* b200track.h -- C ABI of libb200track.so (H100 / sm_90a).
  *
  * The reference (JackWoo0831/Yolov7-tracker) has no FFI: its "operator API" is the Python module
  * surface of tracker/{kalman_filter,matching,basetrack,bytetrack,botsort}.py.  Each entry point
- * below names the reference function it replaces (file:line relative to /root/reference); the
+ * below names the reference function it replaces (file:line relative to the reference tree); the
  * Python drop-in modules under yolov7-tracker_b200/tracker bind them through ctypes
  * (see INTEGRATION.md).
  *
@@ -30,7 +30,7 @@ enum { B2T_F32 = 0, B2T_F64 = 1 };
 enum { B2T_FMT_XYAH = 0, B2T_FMT_XYWH = 1, B2T_FMT_NSA = 2 };
 enum { B2T_SORT = 0, B2T_BYTETRACK = 1, B2T_BOTSORT = 2 };
 enum { B2T_OK = 0, B2T_EINVAL = -1, B2T_ECUDA = -2, B2T_ECAPACITY = -3, B2T_ENOTBUILT = -4 };
-/* 16-bit activation / weight type of the detector branch.  Both feed tcgen05 kind::f16 at the same rate with fp32
+/* 16-bit activation / weight type of the detector branch.  Both feed wgmma at the same rate with fp32
  * accumulation; fp16 (the reference's own GPU half mode, detect.py:41) carries 3 more mantissa bits than bf16. */
 enum { B2T_ACT_BF16 = 0, B2T_ACT_F16 = 1 };
 
@@ -106,6 +106,8 @@ int b2t_tracker_out_cols(void);   /* 8: id, x, y, w, h, cls, score, slot */
 int b2t_tracker_stat_words(void); /* 64: [0..16) counters, [16..32) per-phase SM cycles, [32..64) sub-phase cycles */
 /* One frame for every sequence.
  *   dets      [S][dmax][6] float32  x1,y1,x2,y2,score,cls (what track.py:149 hands to tracker.update)
+ *             a box the reference cannot track is ignored (a deliberate divergence): a non-finite coordinate, y2 == y1, or
+ *             x2 == x1 with the xywh (BoT-SORT) filter -- its Kalman state would turn NaN or its Cholesky factorisation fail
  *   det_count [S] int32
  *   warps     [S][6] float64 or NULL (BoT-SORT camera motion, botsort.py:380)
  *   id_base   [S] int32 or NULL: overrides the sequence's id counter before births (BaseTrack._count)
@@ -126,7 +128,7 @@ int b2t_tracker_read_list(b2t_tracker* t, int seq, int which, double* rows_host,
 /* Copies one slot's Kalman state to the host as float64: mean[8], cov[64] (lazy STrack.mean/.cov). */
 int b2t_tracker_read_slot(b2t_tracker* t, int seq, int slot, double* mean_host, double* cov_host, void* stream);
 
-/* ---------------------------------------------------------------- detector: conv + bias + SiLU (tcgen05 / TMA)
+/* ---------------------------------------------------------------- detector: conv + bias + SiLU (wgmma / TMA)
  * Replaces Conv.fuseforward (models/common.py:110-111, BN folded as utils/torch_utils.py:181-201) and the
  * linear 1x1 convs of Detect (models/yolo.py:44).  Activations NHWC bf16, possibly a channel slice of a wider
  * (concat) buffer; weights [cout_rows][kh][kw][cin] bf16; bias fp32 [cout]; output bf16 or fp32 written at
@@ -150,7 +152,7 @@ typedef struct b2t_conv_desc {
     int out_pitch, out_coff;
     int act;              /* 1 = SiLU, 0 = linear, 2 = ReLU (the ReID extractor, tracker/reid_models/deepsort_reid.py), 3 = LeakyReLU(0.1) (YOLOv7-tiny) */
     int out_f32;          /* 1 = fp32 output, 0 = bf16 */
-    int block_n;          /* 0 = automatic; else output channels per CTA (multiple of 16, <= 256) */
+    int block_n;          /* 0 = automatic; else output channels per CTA (multiple of 16, <= 256; rounded up to 32, 64, 128 or 256) */
     int tile_w;           /* 0 = automatic; else spatial tile width (4, 8 or 16) */
     int stages;           /* 0 = automatic (as deep as shared memory allows); else shared-memory ring depth (1..8) */
     int in_row_pixels;    /* 0 = w; else pixels per input row in memory (rows padded on the right; x points at column 0) */
@@ -172,12 +174,12 @@ typedef struct b2t_conv_desc {
                            * the chunk count is even), 1 = one chunk per stage, 2 = require pairs */
     int out_bufs;         /* epilogue staging boxes (128 pixels x 128 B) per sub-tile: 0 = automatic, 1 or 2 */
     int mt;               /* 0 / 1 = one 128-pixel tile per CTA tile; 2 = two 128-pixel sub-tiles per tile (256 pixels), each weight
-                           * tile that reaches shared memory feeds both: half the weight traffic per flop.  2 x mt x BLOCK_N <= 512. */
+                           * tile that reaches shared memory feeds both: half the weight traffic per flop.  mt x BLOCK_N <= 256 (accumulator registers). */
     int producers;        /* TMA producer warps per CTA: 0 = default (2), 1 or 2.  A thread's bulk-tensor copies complete one after the
                            * other, so a CTA that owns its SM needs several issuing threads to keep the operand ring full. */
     int splits;           /* 0 / 1 = off; k > 1 = split-K: k work units per tile accumulate disjoint K ranges, park fp32 partial sums
                            * in a plan-owned workspace, and the last unit to arrive reduces them in split order (deterministic) and
-                           * runs the epilogue -- for the 20 x 20 / 40 x 40 maps whose tile count cannot fill 148 SMs. */
+                           * runs the epilogue -- for the 20 x 20 / 40 x 40 maps whose tile count cannot fill the SMs. */
 } b2t_conv_desc;
 typedef struct b2t_conv_plan b2t_conv_plan;
 const char* b2t_conv_last_error(void);
@@ -185,12 +187,10 @@ int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_plan);
 void b2t_conv_plan_destroy(b2t_conv_plan* plan);
 double b2t_conv_plan_flops(const b2t_conv_plan* plan);
 /* launch geometry chosen at plan time: out[0..17) = grid, threads, dynamic smem bytes, BLOCK_N, ring stages, mt, splits, halo,
- * halo buffers, tiles_m, tiles_n, TMEM columns, producer warps, taps per stage, resident weights, staging boxes, K chunks per stage (diagnostics for the autotuner and the per-layer tables in profiles/). */
+ * halo buffers, tiles_m, tiles_n, accumulator registers per consumer thread, producer warps, taps per stage, resident weights, staging boxes,
+ * K chunks per stage (diagnostics for the autotuner and the per-layer tables). */
 int b2t_conv_plan_info(const b2t_conv_plan* plan, int* out, int n);
 int b2t_conv_run(const b2t_conv_plan* plan, void* stream);
-/* diagnostic builds (-DB2T_CONV_TRACE): per-CTA cycle counters of the MMA warp [total, ring wait, TMEM wait, halo wait, operand wait,
- * issue] and of the epilogue groups; returns the number of CTAs copied, 0 in normal builds */
-int b2t_conv_plan_trace(const b2t_conv_plan* plan, long long* out_host, int max_ctas);
 
 /* ---------------------------------------------------------------- detector glue + NMS (csrc/b2t_detect.cu) */
 const char* b2t_detect_last_error(void);

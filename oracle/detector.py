@@ -92,6 +92,36 @@ def forward(layers, sd, img, anchors, strides, nc=80, emulate_bf16=False, return
     raise RuntimeError("layer list has no detect layer")
 
 
+def seeded_training_state_dict(keys, shapes, seed):
+    """A seeded state dict for a reference graph given its key names and shapes (no reference code needed): conv weights and
+    biases uniform in +-1/sqrt(fan_in) (torch's default init), BatchNorm statistics / affine randomised, ImplicitA ~ N(0, 0.02),
+    ImplicitM ~ N(1, 0.02), num_batches_tracked 0.  Keys are filled in the given order from ONE generator."""
+    g = torch.Generator().manual_seed(int(seed))
+    shapes = {k: tuple(int(v) for v in s) for k, s in zip(keys, shapes)}
+    sd = {}
+    for k in keys:
+        shp = shapes[k]
+        if k.endswith("num_batches_tracked"):
+            sd[k] = torch.zeros(shp, dtype=torch.int64)
+        elif k.endswith("running_mean"):
+            sd[k] = torch.randn(shp, generator=g) * 0.1
+        elif k.endswith("running_var"):
+            sd[k] = torch.rand(shp, generator=g) * 0.5 + 0.75
+        elif ".bn." in k and k.endswith(".weight"):
+            sd[k] = torch.rand(shp, generator=g) * 0.5 + 1.2
+        elif ".bn." in k and k.endswith(".bias"):
+            sd[k] = torch.randn(shp, generator=g) * 0.1
+        elif ".ia." in k:
+            sd[k] = torch.randn(shp, generator=g) * 0.02
+        elif ".im." in k:
+            sd[k] = 1.0 + torch.randn(shp, generator=g) * 0.02
+        else:
+            w = shapes.get(k[:-len(".bias")] + ".weight") if k.endswith(".bias") else shp
+            fan_in = int(torch.tensor(w[1:]).prod()) if w is not None and len(w) > 1 else 1
+            sd[k] = (torch.rand(shp, generator=g) * 2 - 1) / fan_in ** 0.5
+    return sd
+
+
 def non_max_suppression(prediction, conf_thres=0.25, iou_thres=0.45, max_det=300, max_nms=30000, max_wh=4096):
     """utils/general.py:607-695, best-class branch (multi_label False, classes None, agnostic False)."""
     import torchvision

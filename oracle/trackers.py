@@ -208,14 +208,19 @@ class TrackerOracle:
         dets = np.asarray(dets, dtype=np.float32).reshape(-1, 6)
         sc = dets[:, 4]
         f32 = np.float32
+        tlwh = K.tlbr_to_tlwh_f32(dets[:, :4])
+        # deliberate divergence, limited to boxes the reference cannot track (as in the kernel): a non-finite coordinate, zero height
+        # (xyah: no aspect ratio, zero Kalman noise -> NaN state / failed Cholesky) or, with the xywh filter, zero width takes no part
+        area = np.isfinite(dets[:, :4]).all(1) & (tlwh[:, 3] != 0)
+        if self.fmt == K.FMT_XYWH:
+            area &= tlwh[:, 2] != 0
         if self.kind == "sort":
-            hi = np.nonzero(sc > f32(self.det_thresh))[0]                       # basetrack.py:387
+            hi = np.nonzero(np.logical_and(sc > f32(self.det_thresh), area))[0]  # basetrack.py:387
             lo = np.zeros(0, dtype=np.int64)
         else:
             him = sc >= f32(self.det_thresh)                                    # bytetrack.py:69-70
             lom = np.logical_and(~him, sc > f32(self.low_thresh))
-            hi, lo = np.nonzero(him)[0], np.nonzero(lom)[0]
-        tlwh = K.tlbr_to_tlwh_f32(dets[:, :4])
+            hi, lo = np.nonzero(np.logical_and(him, area))[0], np.nonzero(np.logical_and(lom, area))[0]
         tlbr = tlwh.copy()
         tlbr[:, 2:] += tlbr[:, :2]
         tlbr64 = tlbr.astype(np.float64)

@@ -1,6 +1,6 @@
 """Writes tests/golden/w6_plan.json: the launch plan DetectorW6 builds (every b2t_conv_desc, op order, head levels) for two
-input sizes, recorded WITHOUT a GPU by tests/plan_dryrun.py.  It was written from the build whose plan passed the B200 parity
-tests of round 1 (profiles/r01_pytest_gpu.log), so that later planner changes can be checked against it on CPU.
+input sizes, recorded WITHOUT a GPU by tests/plan_dryrun.py.  It was written from the build whose plan passed the GPU parity
+tests of round 1, so that later planner changes can be checked against it on CPU.
 
     python tests/golden/make_golden_plan.py
 """

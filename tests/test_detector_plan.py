@@ -1,5 +1,5 @@
 """not-gpu: the launch plan DetectorW6 builds (every conv descriptor, the op order, the head levels), recorded on CPU by
-tests/plan_dryrun.py, against (a) the committed plan of the build that passed the round-1 B200 parity tests
+tests/plan_dryrun.py, against (a) the committed plan of the build that passed the round-1 GPU parity tests
 (tests/golden/w6_plan.json) and (b) for non-square inputs, the tensor shapes of the torch oracle."""
 import json
 import os

@@ -1,4 +1,4 @@
-"""-m gpu: the camera-motion estimator (csrc/b2t_gmc.cu, SURVEY.md 8f row 1) on a B200 through the C ABI against oracle/gmc.py
+"""-m gpu: the camera-motion estimator (csrc/b2t_gmc.cu, SURVEY.md 8f row 1) on an H100 through the C ABI against oracle/gmc.py
 (pinned against cv2 and the reference's GMC class by tests/test_oracle_gmc.py): full-size frames, several sequences per call,
 detection masks, rotated / scaled motion, the drop-in ``botsort.GMC`` and ``BoTSORT(use_GMC=True)``, the pipelined two-call form."""
 import os
@@ -174,7 +174,7 @@ def test_pipeline_botsort_with_gpu_gmc_equals_stepwise():
 
 def test_gpu_vs_committed_reference_golden():
     """tests/golden/gmc.npz: the matrices of the UNMODIFIED reference GMC class over two seeded sequences (one of odd size) with masked
-    detections; the B200 estimate moves the frame's corners by less than a pixel differently (the spread of two RANSAC realisations)."""
+    detections; the GPU estimate moves the frame's corners by less than a pixel differently (the spread of two RANSAC realisations)."""
     sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
     from make_golden_gmc import CASES, frames_and_dets
     gold = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "gmc.npz"))

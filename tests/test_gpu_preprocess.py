@@ -75,7 +75,7 @@ def test_letterboxed_frame_through_non_square_detector():
 
 @pytest.mark.parametrize("act", ["fp16", "bf16"])
 def test_letterbox_reorg_fused_on_gpu_equals_two_steps_and_oracle(act):
-    """b2t_letterbox_reorg on the B200 (uint8 BGR frames -> the detector's padded ReOrg / NHWC 16-bit input, one kernel) ==
+    """b2t_letterbox_reorg on the GPU (uint8 BGR frames -> the detector's padded ReOrg / NHWC 16-bit input, one kernel) ==
     b2t_letterbox (float canvas, already pinned bit-exact against the reference's own output) followed by b2t_image_reorg_padded,
     bit for bit, for a resized 1080p frame pair and a same-size frame; and == the oracle's canvas pushed through ReOrg + torch's
     rounding.  Integer resize arithmetic + IEEE division + round-to-nearest-even conversion: tolerance 0."""

@@ -1,4 +1,4 @@
-"""-m gpu: the ReID extractor of the appearance branch (SURVEY.md 8f row 3) on a B200 -- tcgen05 convolutions + the element-wise
+"""-m gpu: the ReID extractor of the appearance branch (SURVEY.md 8f row 3) on an H100 -- wgmma convolutions + the element-wise
 kernels of csrc/b2t_reid.cu -- against oracle/reid.py (pinned against the reference's own Net / Extractor and its checkpoint by
 tests/test_oracle_reid.py).  fp16 activations: features are compared by cosine similarity and absolute difference."""
 import os
@@ -26,7 +26,7 @@ def test_extractor_features_vs_oracle(bn_mode):
     cos = (got * exp).sum(1)
     print("reid %s: min cosine %.6f, max |d| %.2e" % (bn_mode, float(cos.min()), float(np.abs(got - exp).max())))
     assert np.allclose(np.linalg.norm(got, axis=1), 1.0, atol=1e-4)
-    assert cos.min() > 0.9999 and np.abs(got - exp).max() < 2e-3                  # measured on a B200: 0.999999 / 2.2e-4 (fp16 activations)
+    assert cos.min() > 0.9999 and np.abs(got - exp).max() < 2e-3
     # the pre-processing stage on its own: crop -> float / 255 -> bilinear 64 x 128 -> Normalize, fp16-rounded
     x = ext.last_net["x"][:11, :, :, :3].float().cpu().permute(0, 3, 1, 2)
     assert float((x - R.preprocess(crops)).abs().max()) < 3e-3
@@ -35,7 +35,7 @@ def test_extractor_features_vs_oracle(bn_mode):
 
 def test_features_from_frame_and_cosine_distance():
     """BoTSORT.get_feature's form (crops = windows of the frame, botsort.py:291-311) and the distance matrix of
-    matching.embedding_distance (matching.py:84-103) on the tcgen05 GEMM."""
+    matching.embedding_distance (matching.py:84-103) on the wgmma conv kernel."""
     from b200track.gemm import CosineGemm
     from b200track.synth import textured_frame
     sd = R.seeded_state_dict(4)

@@ -1,5 +1,5 @@
 """-m gpu: YOLOv7-tiny (BASELINE.json configs[0]: cfg/deploy/yolov7-tiny.yaml -- LeakyReLU convs, MP / SP pools, three Detect levels)
-on the B200 kernels against oracle/detector.py, which tests/test_oracle_detector.py pins against the reference's own Model."""
+on the GPU kernels against oracle/detector.py, which tests/test_oracle_detector.py pins against the reference's own Model."""
 import pytest
 
 pytestmark = pytest.mark.gpu

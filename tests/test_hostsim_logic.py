@@ -1,6 +1,6 @@
 """not-gpu: kernel LOGIC of csrc/b2t_*.cuh, executed by the fiber simulator (tests/hostsim), against
-the oracle and the committed reference goldens.  This tier exists because the build container
-has no GPU; it does not replace the `-m gpu` parity tests, which run the nvcc build on a B200."""
+the oracle and the committed reference goldens.  This tier exists because the CPU test machine
+has no GPU; it does not replace the `-m gpu` parity tests, which run the nvcc build on an H100."""
 import ctypes as C
 import os
 import sys
@@ -12,7 +12,7 @@ sys.path.insert(0, os.path.join(os.path.dirname(__file__), "hostsim"))
 import simlib  # noqa: E402
 from simlib import ptr, sim, SimTracker  # noqa: E402
 from b200track import _lib as L  # noqa: E402
-from b200track.synth import make_stream  # noqa: E402
+from b200track.synth import make_stream, with_flat_boxes, zero_width_stream  # noqa: E402
 from oracle import kalman as K, iou as oiou, lapjv as olap, trackers as T  # noqa: E402
 
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
@@ -162,6 +162,38 @@ def test_fused_step_matches_reference_golden(kind, case):
         if i in keep:
             k = keep[i]
             np.testing.assert_allclose(res[i][:, 1:5], g[case + "_tlwh"][tl_off[k]:tl_off[k + 1]], rtol=1e-9, atol=1e-9)
+
+
+@pytest.mark.parametrize("kind", ["sort", "bytetrack", "botsort"])
+def test_fused_step_ignores_boxes_without_area(kind):
+    """Detections the reference cannot track -- zero height, non-finite coordinates, and with the xywh filter (BoT-SORT) zero width:
+    its Kalman state would turn NaN or its Cholesky factorisation fail -- take no part: the tracks equal those of the stream without
+    them, and every output is finite."""
+    frames, warps = make_stream(41, 10, 40, warp_sigma=3.0 if kind == "botsort" else 0.0)
+    rng = np.random.default_rng(5)
+    dirty = [with_flat_boxes(f, rng, xywh=kind == "botsort") for f in frames]
+    res, _ = _run_loop(kind, dirty, warps, cap=256, dmax=128)
+    orc = T.TrackerOracle(kind)
+    for i, f in enumerate(frames):
+        exp = orc.update(f, warps[i] if kind == "botsort" else None)
+        assert np.isfinite(res[i]).all(), "frame %d" % (i + 1)
+        assert [int(v) for v in res[i][:, 0]] == [e[0] for e in exp], "frame %d" % (i + 1)
+        if exp:
+            np.testing.assert_allclose(res[i][:, 1:5], np.array([e[1] for e in exp]), rtol=1e-9, atol=1e-9)
+
+
+@pytest.mark.parametrize("kind", ["sort", "bytetrack"])
+def test_fused_step_tracks_zero_width_boxes_like_reference(kind):
+    """Zero-width, positive-height boxes are defined for the xyah filter and the reference tracks them: the kernel gives the
+    reference's ids (tests/golden/refchecks.npz) on every frame and its boxes on the last."""
+    g = np.load(os.path.join(GOLDEN, "refchecks.npz"))
+    counts = g["flat_%s_count" % kind]
+    off = np.concatenate([[0], np.cumsum(counts)])
+    frames = zero_width_stream(61, len(counts), 60)
+    res, _ = _run_loop(kind, frames, None, cap=256, dmax=128)
+    for i in range(len(frames)):
+        assert res[i][:, 0].astype(np.int64).tolist() == g["flat_%s_ids" % kind][off[i]:off[i + 1]].tolist(), "frame %d" % (i + 1)
+    np.testing.assert_allclose(res[-1][:, 1:5], g["flat_%s_tlwh_last" % kind], rtol=1e-9, atol=1e-9)
 
 
 def test_fused_step_two_sequences_and_id_base():

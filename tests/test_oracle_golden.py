@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 
 from oracle import kalman as K, trackers as T, iou as oiou, lapjv as olap
-from b200track.synth import make_stream, stream_digest
+from b200track.synth import make_stream, stream_digest, zero_width_stream
 
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
 
@@ -103,3 +103,17 @@ def test_linear_assignment_empty_sides():
     assert m.shape == (0, 2) and ua == () and ub == (0, 1, 2, 3, 4)
     m, ua, ub = olap.linear_assignment(np.zeros((3, 0)), 0.9)
     assert m.shape == (0, 2) and ua == (0, 1, 2) and ub == ()
+
+
+@pytest.mark.parametrize("kind", ["sort", "bytetrack"])
+def test_oracle_tracks_zero_width_boxes_like_reference(kind):
+    """Boxes flattened to zero width (x2 = x1, height kept) are defined for the xyah Kalman filter -- aspect ratio 0 -- and the
+    reference tracks them: the oracle gives the reference's ids on every frame and its boxes on the last (tests/golden/refchecks.npz)."""
+    g = _load("refchecks.npz")
+    orc = T.TrackerOracle(kind)
+    counts = g["flat_%s_count" % kind]
+    off = np.concatenate([[0], np.cumsum(counts)])
+    for i, f in enumerate(zero_width_stream(61, len(counts), 60)):
+        exp = orc.update(f)
+        assert [e[0] for e in exp] == g["flat_%s_ids" % kind][off[i]:off[i + 1]].tolist(), "frame %d" % (i + 1)
+    np.testing.assert_allclose(np.array([e[1] for e in exp]), g["flat_%s_tlwh_last" % kind], rtol=1e-9, atol=1e-9)

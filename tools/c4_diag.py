@@ -1,5 +1,5 @@
 import os, sys, numpy as np, torch
-ROOT = os.environ.get("GRAFT_REPO_ROOT", "/root/repo")
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "yolov7-tracker_b200"))
 from b200track import _lib as L
 from b200track.detector import DetectorW6

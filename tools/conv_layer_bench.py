@@ -1,4 +1,4 @@
-"""GPU box: per-layer sweep of the tcgen05 conv kernel's tiling modes on the YOLOv7-w6 shapes (batch 8, 1280 x 1280).
+"""GPU box: per-layer sweep of the wgmma conv kernel's tiling modes on the YOLOv7-w6 shapes (batch 8, 1280 x 1280).
 
 For every layer in LAYERS and every valid (halo, mt, BLOCK_N, ring depth, K splits): checks the output against torch
 (F.conv2d on the same fp16-rounded operands, fp32 accumulation) and times `reps` back-to-back launches with CUDA events.

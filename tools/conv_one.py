@@ -1,4 +1,4 @@
-"""GPU box: run ONE configuration of one w6 layer a few times (for ncu).  python tools/conv_one.py L23 halo=1 mt=1 bn=256 stages=0 producers=2 splits=1"""
+"""GPU box: run ONE configuration of one w6 layer a few times (for a profiler).  python tools/conv_one.py L23 halo=1 mt=1 bn=256 stages=0 producers=2 splits=1"""
 import os
 import sys
 

@@ -1,4 +1,4 @@
-"""GPU: TFLOP/s of the tcgen05 conv kernel on the dominant YOLOv7-w6 shapes (batch 8) + whole-forward timing."""
+"""GPU: TFLOP/s of the wgmma conv kernel on the dominant YOLOv7-w6 shapes (batch 8) + whole-forward timing."""
 import os, sys, json
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "yolov7-tracker_b200"))

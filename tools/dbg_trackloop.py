@@ -1,5 +1,5 @@
 """GPU box: the loop of tests/test_gpu_trackloop.py, repeated with freshly tuned detectors; on a divergence from the oracle the
-sequence's detections go to gpurun_out/trackloop_fail_<k>.npz (replayable on CPU through the host simulator)."""
+sequence's detections go to trackloop_out/trackloop_fail_<k>.npz (replayable on CPU through the host simulator)."""
 import os
 import sys
 
@@ -68,7 +68,8 @@ def run(k):
                         print("   row %d id %d gpu %s oracle %s" % (r, cid[r], a[r], b[r]))
                 else:
                     print("   ids gpu", cid[:40]); print("   ids orc", eid[:40])
-                np.savez(os.path.join(ROOT, "gpurun_out", "trackloop_fail_%d_%s.npz" % (k, name)), id0=id0, **{"f%d" % i: h for i, h in enumerate(hist)})
+                os.makedirs(os.path.join(ROOT, "trackloop_out"), exist_ok=True)
+                np.savez(os.path.join(ROOT, "trackloop_out", "trackloop_fail_%d_%s.npz" % (k, name)), id0=id0, **{"f%d" % i: h for i, h in enumerate(hist)})
                 break
     print("run %d: %s" % (k, "DIVERGED" if bad else "ok"))
     return bad

@@ -2,7 +2,7 @@
 
 The reference saves / loads whole ``nn.Module`` objects: ``attempt_load`` does ``ckpt = torch.load(w); model = ckpt['ema' if
 ckpt.get('ema') else 'model'].float().fuse().eval()`` (models/experimental.py:83-106).  Un-pickling needs the reference's own
-``models`` / ``utils`` packages on ``sys.path``; the B200 detector only needs the tensors.  This script does the reference's own
+``models`` / ``utils`` packages on ``sys.path``; the GPU detector only needs the tensors.  This script does the reference's own
 load + ``.float()`` and writes ``model.state_dict()`` -- deploy, unfused (Conv + BN) or training-graph (IAuxDetect) naming, all of
 which ``b200track.w6.fold_reference_state_dict`` folds on load:
 

@@ -7,7 +7,6 @@
     16 (N + M) and writes e N M; LAP reads the matrix once (e N M).
   * Kalman predict / update / multi_gmc over 1 M tracks: 144 e / 148 e / 144 e bytes per track (e = 4 or 8).
 Every kernel is timed with CUDA events after warm-up, L2 flushed between repetitions; GB/s against MEASURED_PEAKS.json.
-Written at the end of round 1 (no GPU minutes left to run it): the numbers belong to round 2's profiles/.
 """
 import argparse
 import json

@@ -1,4 +1,4 @@
-"""GPU box: how far is the tcgen05 detector from the fp32 oracle, per activation type and input size?
+"""GPU box: how far is the wgmma detector from the fp32 oracle, per activation type and input size?
 
 For every (size, batch) and act_dtype in {fp16, bf16}: raw-logit error against the oracle that emulates the same 16-bit rounding
 and against the pure fp32 oracle, objectness error, and the post-NMS agreement SURVEY 7.2 #5 defines (kept boxes with an fp32

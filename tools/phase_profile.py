@@ -46,6 +46,6 @@ if __name__ == "__main__":
         sub = st[:, :, L.STAT_SUB0:L.STAT_SUB0 + 16].astype(np.float64).mean(axis=(0, 1))
         print("   csr1 sub: colstats %.0f | sort %.0f | count %.0f | scan %.0f | list %.0f | iou %.0f" % tuple(sub[:6]))
         print("   lap1 sub: init %.0f | kernelize %.0f | compact %.0f | labels %.0f | solve %.0f" % tuple(sub[8:13]))
-    for S in (1, 4, 148):
+    for S in (1, 4, 132):
         ms, ph, st = run(kind, S, "f64", frames=30)
         print("S=%4d  %.1f us/step  %.0f frames/s" % (S, ms * 1e3, S / ms * 1e3))

@@ -8,8 +8,7 @@ import ctypes as C
 import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-# B2T_LIB_PATH: diagnostic twin of the library (build.py --trace), never a different implementation
-LIB_PATH = os.environ.get("B2T_LIB_PATH") or os.path.join(HERE, "libb200track.so")
+LIB_PATH = os.path.join(HERE, "libb200track.so")
 
 F32, F64 = 0, 1
 FMT_XYAH, FMT_XYWH, FMT_NSA = 0, 1, 2
@@ -75,7 +74,6 @@ SIGNATURES = {
     "b2t_conv_plan_flops": (C.c_double, [_P]),
     "b2t_conv_plan_info": (_I, [_P, C.POINTER(C.c_int), _I]),
     "b2t_conv_run": (_I, [_P, _P]),
-    "b2t_conv_plan_trace": (_I, [_P, C.POINTER(C.c_longlong), _I]),
     "b2t_detect_last_error": (C.c_char_p, []),
     "b2t_image_reorg": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "b2t_image_reorg_padded": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),

@@ -1,4 +1,4 @@
-"""Host side of the tcgen05 conv kernel (csrc/b2t_conv.cu): weight packing and plan objects.
+"""Host side of the wgmma conv kernel (csrc/b2t_conv.cu): weight packing and plan objects.
 
 ``pack_conv_weight`` turns a (BN-folded) ``[Cout, Cin, KH, KW]`` fp32 weight into the K-major
 ``[Cout_rows, KH, KW, Cin_pad]`` bf16 layout the B-operand tensor map reads.  ``ConvPlan`` owns the
@@ -54,7 +54,7 @@ class ConvPlan:
         self.flops = self.lib.b2t_conv_plan_flops(self.handle)
         info = (C.c_int * 17)()
         self.lib.b2t_conv_plan_info(self.handle, info, 17)
-        self.info = dict(zip(("grid", "threads", "smem", "bn", "stages", "mt", "splits", "halo", "halo_bufs", "tiles_m", "tiles_n", "tmem_cols", "producers", "tps", "b_res", "out_bufs", "kpair"), list(info)))
+        self.info = dict(zip(("grid", "threads", "smem", "bn", "stages", "mt", "splits", "halo", "halo_bufs", "tiles_m", "tiles_n", "acc_regs", "producers", "tps", "b_res", "out_bufs", "kpair"), list(info)))
 
     def run(self, stream=None):
         s = C.c_void_p(torch.cuda.current_stream().cuda_stream if stream is None else stream)

@@ -1,11 +1,11 @@
-"""YOLOv7-w6 forward + decode + NMS on the B200 kernels (csrc/b2t_conv.cu, csrc/b2t_detect.cu).
+"""YOLOv7-w6 forward + decode + NMS on the H100 kernels (csrc/b2t_conv.cu, csrc/b2t_detect.cu).
 
 Replaces, for the reference's detector boundary (SURVEY.md section 8b B-det):
   ``model(img)[0]``                     models/yolo.py:321-351 (forward_once) + :39-57 (Detect)
   ``non_max_suppression(...)``          utils/general.py:607-695
   ``scale_coords(...).round()``         utils/general.py:319-340, tracker/track.py:240
 
-Activations are NHWC bf16 with fp32 accumulation in TMEM; the Detect logits stay fp32.  Every tensor that feeds a
+Activations are NHWC bf16 with fp32 accumulation in registers; the Detect logits stay fp32.  Every tensor that feeds a
 ``Concat`` is produced at its channel offset inside the concat buffer (no copies); the whole forward is a fixed
 sequence of ~115 launches, optionally replayed as one CUDA graph.  ``detect()`` never materialises the (B, N, 85)
 prediction tensor: the decode is fused into the NMS candidate filter; ``forward()`` / ``decode()`` produce it on request.
@@ -34,7 +34,7 @@ class DetectorW6:
         """layers / anchors / strides / act: the graph (default: YOLOv7-w6, SiLU).  ``b200track.tiny.DetectorTiny`` passes the
         YOLOv7-tiny graph (LeakyReLU(0.1) = act 3, MP / SP pools, three Detect levels, total stride 32)."""
         if not torch.cuda.is_available():
-            raise L.B2TError("DetectorW6 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+            raise L.B2TError("DetectorW6 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         # img_size: int (square) or (height, width) -- e.g. the 768 x 1280 minimum rectangle a letterboxed 1080p frame becomes
         H, W = (img_size, img_size) if isinstance(img_size, int) else (int(img_size[0]), int(img_size[1]))
         assert H % total_stride == 0 and W % total_stride == 0, "image sides must be multiples of the graph's total stride (w6: 64 = ReOrg / 2 and five stride-2 convs)"
@@ -42,7 +42,7 @@ class DetectorW6:
         no_ = name_offset              # layer index -> the reference's module index (the tiny graph has an explicit input op in front)
         self.lib = L.load()
         # 16-bit type of activations and weights: fp16 (default; the reference's own GPU half mode, detect.py:41) or bf16 --
-        # the same tcgen05 kind::f16 rate, fp32 accumulation either way; fp16 keeps 3 more mantissa bits, bf16 the fp32 range
+        # the same wgmma rate, fp32 accumulation either way; fp16 keeps 3 more mantissa bits, bf16 the fp32 range
         self.act_dtype = act_dtype
         self.act_code = L.act_dtype_code(act_dtype)
         self.dev = torch.device(device)
@@ -259,7 +259,8 @@ class DetectorW6:
             shapes = [dict(block_n=bn, mt=mt, stages=st, kpair=kp) for bn in (64, 128, 256) for mt in (1, 2) for st in (0, 2, 3) for kp in kpairs
                       if bn <= max(64, cout_pad) and 2 * mt * bn <= 512 and not (f32 and mt == 2 and bn > 64)]
         # one tuning per process and layer signature: a second detector of the same shape (tests, the bench's arms) gets the SAME
-        # plans -- tile shape and addressing variant decide the fp32 summation order, so independently tuned twins differ in the last bit
+        # plans without a second tuning pass.  (Every candidate sums each output in the same order -- csrc/b2t_conv.cu -- so the
+        # choice changes the time, not the result.)
         key = (str(self.dev), self.B, tuple(hw_in), cin, cout, k, s, bool(act), bool(f32), str(src[0].dtype), src[0].shape[-1], src[1], dst[0].shape[-1], dst[1],
                tuple(tuple(sorted(e.items())) for _, e in variants))
         if self.autotune and key in _TUNE_CACHE:

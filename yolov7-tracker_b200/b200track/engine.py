@@ -20,7 +20,7 @@ class TrackEngine:
     def __init__(self, kind="bytetrack", n_seq=1, dtype="f64", cap=1024, dmax=1024, ecap=None, kalman_format=None,
                  conf_thresh=0.2, iou_thresh=0.5, track_buffer=30, frame_rate=30, use_gmc=True, device="cuda:0"):
         if not torch.cuda.is_available():
-            raise L.B2TError("TrackEngine needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+            raise L.B2TError("TrackEngine needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.lib = L.load()
         self.device = torch.device(device)
         if self.device.type == "cuda" and self.device.index is None:

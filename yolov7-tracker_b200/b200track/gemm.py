@@ -1,4 +1,4 @@
-"""Cosine-similarity GEMM of the appearance branch on the tcgen05 kernel (SURVEY.md section 8f row 3).
+"""Cosine-similarity GEMM of the appearance branch on the wgmma conv kernel (SURVEY.md section 8f row 3).
 
 ``matching.embedding_distance`` / ``cal_cosine_distance`` (tracker/matching.py:84-103, 165-178) compute
 ``normalize(tracks) @ normalize(detections).T`` -- an N x 512 x M contraction, the one genuine tensor-core GEMM on the association

@@ -1,9 +1,9 @@
 """detect -> NMS -> associate as one pipelined object: what ``tracker/track.py:138-179`` does per frame
 (model forward, non_max_suppression + scale_coords, tracker.update), for B sequences at once.
 
-CUDA streams keep the B200 busy across frames:
+CUDA streams keep the GPU busy across frames:
   copy    : pinned host frames -> device, then the uint8 ingest kernel (letterbox + RGB + /255 + ReOrg + 16-bit NHWC)
-  detect  : the 107 tcgen05 convs + glue of the forward (one CUDA graph per detector), back to back
+  detect  : the 107 wgmma convs + glue of the forward (one CUDA graph per detector), back to back
   nms     : Detect decode fused with NMS (second graph)
   track   : [camera-motion estimate] + fused ByteTrack / SORT / BoT-SORT step on the NMS output, then D2H of the track rows
 With ONE detector the ingest and the NMS share the detect stream (its input, head and output buffers are single).  With TWO twin

@@ -2,7 +2,7 @@
 
 ``ReidExtractor`` runs the reference's ReID network (tracker/reid_models/deepsort_reid.py:63-106 ``Net(reid=True)``: conv 3->64 + BN +
 ReLU + max-pool, four stages of two ``BasicBlock``s (:14-49), 8 x 4 average pool, L2 normalisation -> 512-d unit vectors) on crops of
-64 x 128 pixels: the 20 convolutions (+ folded BatchNorm + ReLU) are plans of the tcgen05 conv kernel (csrc/b2t_conv.cu, act = 2),
+64 x 128 pixels: the 20 convolutions (+ folded BatchNorm + ReLU) are plans of the wgmma conv kernel (csrc/b2t_conv.cu, act = 2),
 the crop / resize / normalise step, the max-pool, the residual add + ReLU and the average pool + norm are the element-wise kernels of
 csrc/b2t_reid.cu.  NHWC fp16 activations, fp32 accumulation -- the same numerics as the detector branch.
 Weights: the ``net_dict`` of the reference's checkpoint (weights/ckpt.t7), or any state dict with the same keys.

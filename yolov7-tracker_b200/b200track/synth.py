@@ -93,3 +93,37 @@ def textured_frame(seed, height=720, width=1280, n_rect=400):
     g = np.clip(img, 0, 255)
     bgr = np.stack([g * 0.9 + 10, g, g * 0.8 + 25], -1)
     return np.clip(bgr, 0, 255).astype(np.uint8)
+
+
+def with_flat_boxes(frame, rng, xywh=False):
+    """The frame's detections plus boxes the tracker ignores (zero height, a point, a NaN box; with the xywh Kalman filter also zero width),
+    high and low scores, inserted at random places; the frame's own detections keep their order."""
+    src = frame[rng.choice(len(frame), 4)].astype(np.float32)
+    bad = src.copy()
+    bad[0, 3] = bad[0, 1]                                   # zero height (a box clipped flat against the top / bottom edge)
+    bad[1, 2], bad[1, 3] = bad[1, 0], bad[1, 1]             # a point
+    bad[2, :4] = np.nan
+    bad[3, 3] = bad[3, 1]
+    if xywh:
+        bad[3, 3], bad[3, 2] = bad[3, 1] + 20.0, bad[3, 0]   # zero width: no noise scale for x / w under xywh
+    bad[:, 4] = np.array([0.9, 0.8, 0.9, 0.3], np.float32)
+    out = frame.astype(np.float32)
+    for row in bad:
+        out = np.insert(out, int(rng.integers(0, len(out) + 1)), row, axis=0)
+    return out
+
+
+def with_zero_width(frame, rng, frac=0.15):
+    """A copy of the frame with a fraction of its boxes flattened to zero width (x2 = x1, the height kept): what scale_coords' clip
+    makes of a box wholly beyond the left or right image edge.  The reference tracks such boxes (xyah filter: aspect ratio 0)."""
+    out = np.array(frame, dtype=np.float32, copy=True)
+    sel = rng.random(len(out)) < frac
+    out[sel, 2] = out[sel, 0]
+    return out
+
+
+def zero_width_stream(seed, n_frames, n_obj):
+    """make_stream(seed, ...) with every frame passed through with_zero_width (generator seeded with the same seed)."""
+    frames, _ = make_stream(seed, n_frames, n_obj)
+    rng = np.random.default_rng(seed)
+    return [with_zero_width(f, rng) for f in frames]

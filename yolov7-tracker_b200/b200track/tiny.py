@@ -1,9 +1,9 @@
-"""YOLOv7-tiny (deploy form) on the B200 detector branch -- BASELINE.json configs[0] names it.
+"""YOLOv7-tiny (deploy form) on the H100 detector branch -- BASELINE.json configs[0] names it.
 
 The reference builds it from ``cfg/deploy/yolov7-tiny.yaml`` (77 modules + Detect): ``Conv`` with ``nn.LeakyReLU(0.1)`` (:15),
 ``MP`` = 2 x 2 max-pool (models/common.py:30-35), ``SP`` = stride-1 max-pools 5 / 9 / 13 (:38-45), ``Concat``, ``nn.Upsample``, and a
 three-level ``Detect`` (strides 8 / 16 / 32).  Same planner and kernels as the w6 graph (``DetectorW6``): every conv one launch of the
-tcgen05 kernel (LeakyReLU in the epilogue: act = 3), concat by address, the three SP pools one launch, MP one element-wise kernel.
+wgmma conv kernel (LeakyReLU in the epilogue: act = 3), concat by address, the three SP pools one launch, MP one element-wise kernel.
 Layer tuples as in ``w6.py``; index 0 is an explicit ``input`` op (float image -> NHWC 16-bit), so layer i is the reference's module i - 1.
 """
 from .detector import DetectorW6

@@ -1,10 +1,10 @@
-"""YOLOv7-w6 graph (deploy form) for the B200 detector branch.
+"""YOLOv7-w6 graph (deploy form) for the H100 detector branch.
 
 The reference builds this network from ``cfg/deploy/yolov7-w6.yaml`` through ``parse_model``
 (models/yolo.py:443-520) and runs it module by module (``Model.forward_once`` :321-351).  Here the
 same 119-layer DAG is generated programmatically (``w6_layers``), a planner assigns every tensor a
 place in an NHWC bf16 buffer -- tensors that feed a ``Concat`` are produced straight into the concat
-buffer (concat-by-address, no copy) -- and every ``Conv`` becomes one launch of the tcgen05 kernel.
+buffer (concat-by-address, no copy) -- and every ``Conv`` becomes one launch of the wgmma conv kernel.
 
 Layer tuple: (index, op, from, args).  ops: 'reorg', 'conv' (cout, k, s), 'concat', 'up', 'sppcspc' (cout), 'detect'.
 Weights use the reference's fused state-dict names (``model.{i}.conv.weight`` / ``.bias``,
@@ -252,8 +252,7 @@ def calibrated_state_dict(seed=0, img_size=1280, device="cuda", obj_mean=-6.5, o
     up (80 % of the anchors pass conf_thres) while at 256 x 256 they are fine.  Init-time plumbing in plain torch
     (fp32); returns the fused-name state dict that the CUDA path, the oracle and the CPU baseline all load.
     ``act_std``: pre-activation standard deviation every conv is scaled to.  1.0 (default, the bench weights) puts SiLU in its
-    non-linear range: a random 60-layer net then amplifies a 1e-4 perturbation ~30x by the head (chaotic regime; measured,
-    profiles/r02_parity_probe_*.jsonl).  0.5 keeps SiLU close to linear -- perturbations are not amplified -- and is what the
+    non-linear range: a random 60-layer net then amplifies a 1e-4 perturbation ~30x by the head (chaotic regime).  0.5 keeps SiLU close to linear -- perturbations are not amplified -- and is what the
     tight detector-parity test uses to tell kernel errors from the network's own sensitivity."""
     import torch.nn.functional as F
     sd = {k: v.to(device) for k, v in seeded_state_dict(seed).items()}

@@ -1,8 +1,7 @@
-"""Builds libb200track.so (sm_100a) in-tree with nvcc.  ``python yolov7-tracker_b200/build.py``.
+"""Builds libb200track.so (H100, sm_90a) in-tree with nvcc.  ``python yolov7-tracker_b200/build.py``.
 
-The library is git-ignored but travels to the GPU box with the gpurun snapshot.  nvcc
-cross-compiles without a GPU, so this also runs in the build container
-(``__graft_entry__.build()`` calls it).
+The library is a git-ignored build product.  nvcc cross-compiles without a GPU, so this also runs on a
+machine without one (``__graft_entry__.build()`` calls it).
 """
 import hashlib
 import os
@@ -14,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "b200track", "libb200track.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC"]
 
 # (source, extra flags).  The tracker TU is built without FMA contraction so that its fp64
@@ -42,21 +41,18 @@ def _sources_digest():
     return h.hexdigest()
 
 
-def build(force=False, verbose=False, trace=False):
-    """Compile every translation unit and link the shared library.  Returns the library path.
-    trace=True builds the diagnostic twin libb200track_trace.so (-DB2T_CONV_TRACE: cycle counters in the conv kernel's MMA
-    and epilogue warps, read by tools/conv_trace.py through B2T_LIB_PATH); the product library never carries them."""
-    lib = LIB.replace(".so", "_trace.so") if trace else LIB
-    bdir = os.path.join(HERE, "build_trace" if trace else "build")
-    stamp = lib + ".stamp"
+def build(force=False, verbose=False):
+    """Compile every translation unit and link the shared library.  Returns the library path."""
+    stamp = LIB + ".stamp"
     digest = _sources_digest()
-    if not force and os.path.exists(lib) and os.path.exists(stamp) and open(stamp).read() == digest:
-        return lib
+    if not force and os.path.exists(LIB) and os.path.exists(stamp) and open(stamp).read() == digest:
+        return LIB
     objs = []
+    bdir = os.path.join(HERE, "build")
     os.makedirs(bdir, exist_ok=True)
     for src, extra in UNITS:
         obj = os.path.join(bdir, src.replace(".cu", ".o"))
-        cmd = [NVCC] + ARCH + COMMON + extra + ["-DB2T_CONV_TRACE"] * int(trace) + ["-Xptxas", "-v"] * int(verbose) + ["-c", os.path.join(CSRC, src), "-o", obj]
+        cmd = [NVCC] + ARCH + COMMON + extra + ["-Xptxas", "-v"] * int(verbose) + ["-c", os.path.join(CSRC, src), "-o", obj]
         if verbose:
             print(" ".join(cmd))
         r = subprocess.run(cmd, capture_output=True, text=True)
@@ -65,52 +61,14 @@ def build(force=False, verbose=False, trace=False):
         if r.returncode != 0:
             raise RuntimeError("nvcc failed for %s:\n%s\n%s" % (src, r.stdout, r.stderr))
         objs.append(obj)
-    cmd = [NVCC] + ARCH + ["-shared", "-o", lib] + objs + ["-lcudart"]
+    cmd = [NVCC] + ARCH + ["-shared", "-o", LIB] + objs + ["-lcudart"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))
     with open(stamp, "w") as f:
         f.write(digest)
-    return lib
-
-
-def sass_counts(out_path=None):
-    """cuobjdump -sass of the built library: per kernel, how many tcgen05 / TMA / TMEM instructions it contains (the SASS mnemonics
-    of tcgen05.mma, tcgen05.ld, cp.async.bulk.tensor loads / stores, elect.sync) -- the evidence file profiles/r02_sass_counts.txt."""
-    import re
-    txt = subprocess.run(["/usr/local/cuda/bin/cuobjdump", "-sass", LIB], capture_output=True, text=True).stdout
-    pats = ["UTCHMMA", "UTCBAR", "LDTM", "UTMALDG", "UTMASTG", "ELECT", "SYNCS", "MUFU.TANH", "HMMA"]
-    rows, cur = [], None
-    for line in txt.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            cur = {"name": m.group(1), "n": 0, **{p_: 0 for p_ in pats}}
-            rows.append(cur)
-            continue
-        if cur is None or "/*" not in line:
-            continue
-        cur["n"] += 1
-        for p_ in pats:
-            if re.search(r"\b" + re.escape(p_) + r"(\.|\b)", line):
-                cur[p_] += 1
-    demangle = subprocess.run(["/usr/local/cuda/bin/cu++filt"] + [r["name"] for r in rows], capture_output=True, text=True).stdout.splitlines() if rows else []
-    lines = ["# cuobjdump -sass yolov7-tracker_b200/b200track/libb200track.so (sm_100a): instruction counts per kernel.",
-             "# UTCHMMA = tcgen05.mma, UTCBAR = tcgen05.commit, LDTM = tcgen05.ld, UTMALDG / UTMASTG = cp.async.bulk.tensor load / store (TMA),",
-             "# SYNCS = mbarrier ops, HMMA = legacy mma.sync (must be 0).  " + "%-64s %7s " % ("kernel", "instrs") + " ".join("%9s" % p_ for p_ in pats)]
-    for r, d in zip(rows, demangle or [r["name"] for r in rows]):
-        d = d.replace("<unnamed>::", "").replace("(anonymous namespace)::", "")
-        short = (d.split("(CUtensorMap")[0].replace("(bool)", "").replace("(int)", "") if "(CUtensorMap" in d else d.split("(")[0])[:64]
-        lines.append("%-64s %7d " % (short, r["n"]) + " ".join("%9d" % r[p_] for p_ in pats))
-    text = "\n".join(lines) + "\n"
-    if out_path:
-        with open(out_path, "w") as f:
-            f.write(text)
-    return text
+    return LIB
 
 
 if __name__ == "__main__":
-    if "--sass" in sys.argv:
-        build()
-        print(sass_counts(os.path.join(os.path.dirname(HERE), "profiles", "r02_sass_counts.txt")))
-        sys.exit(0)
-    print(build(force="--force" in sys.argv, verbose="-v" in sys.argv, trace="--trace" in sys.argv))
+    print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))

@@ -1,4 +1,4 @@
-// b2t_conv.cu -- conv2d + bias + SiLU as an implicit GEMM on the 5th-gen tensor cores (sm_100a).
+// b2t_conv.cu -- conv2d + bias + SiLU as an implicit GEMM on the Hopper tensor cores (sm_90a: TMA + wgmma).
 //
 // Replaces ``Conv.fuseforward`` (models/common.py:110-111: act(conv(x)) with BN folded by
 // utils/torch_utils.py:181-201) and the linear 1x1 head convs of ``Detect`` (models/yolo.py:44)
@@ -6,30 +6,27 @@
 //
 //   D[pixel, cout] = sum_{kh,kw,cin} X[n, ho*s+kh-p, wo*s+kw-p, cin] * W[cout, kh, kw, cin]
 //
-// Layout: activations NHWC bf16 (a tensor may be a channel slice of a wider concat buffer: pitch !=
-// C), weights [Cout][KH][KW][Cin] bf16 (K-major), bias fp32, accumulation fp32 in TMEM.
+// Layout: activations NHWC bf16 / fp16 (a tensor may be a channel slice of a wider concat buffer: pitch !=
+// C), weights [Cout][KH][KW][Cin] (K-major), bias fp32, accumulation fp32 in registers.
 //
-// One CTA computes a 128-pixel x BLOCK_N-channel output tile:
-//   * the 128 pixels are a TH x TW spatial patch of one image (TH*TW = 128).  For filter tap
+// One CTA computes tiles of MT x 128 pixels x BLOCK_N channels:
+//   * the 128 pixels of a sub-tile are a TH x TW spatial patch of one image (TH*TW = 128).  For filter tap
 //     (kh,kw) and channel chunk kc the A operand is ONE TMA box {BK ch, TW, TH, 1} of the 4-D
 //     tensor map (C, W, H, N) at coordinates (kc*BK, wo0*s+kw-p, ho0*s+kh-p, n): out-of-bounds
 //     rows/cols are zero-filled by the TMA unit (that IS the padding), stride-2 convs use the tensor
 //     map's element strides, and the box lands in shared memory as 128 rows of BK*2 bytes with the
-//     128-/64-/32-byte swizzle -- exactly the canonical K-major UMMA operand layout.  No im2col.
+//     128-/64-/32-byte swizzle -- exactly the canonical K-major wgmma operand layout.  No im2col.
 //   * B operand: 2-D map (K, Cout), box {BK, BLOCK_N}.
-//   * warp 0 = TMA producer, warp 1 = MMA issuer (one elected thread, tcgen05.mma
-//     cta_group::1 kind::f16, M=128, N=BLOCK_N, K=16 per instruction), warps 2..5 = epilogue:
-//     tcgen05.ld 32 lanes x 32 columns -> +bias -> SiLU (one tanh.approx on the SFU) -> fp16 / bf16 (or fp32) -> 128-byte-swizzled
+//   * warps [0, 8 MT) are the consumers: two warpgroups per 128-pixel sub-tile, each issuing
+//     wgmma.mma_async m64 x BLOCK_N x k16 on its 64 pixel rows with the accumulator in registers, then the epilogue
+//     from those registers: +bias -> SiLU (one tanh.approx on the SFU) -> fp16 / bf16 (or fp32) -> 128-byte-swizzled
 //     staging tile -> TMA bulk tensor STORES straight into the consumer's concat buffer
-//     (concat-by-address; partial tiles and the 255-channel head are clipped by the TMA unit).  Per-lane 16-byte
-//     global stores at pixel pitch were measured 2-4x slower than the whole MMA pipeline (profiles/).
+//     (concat-by-address; partial tiles and the 255-channel head are clipped by the TMA unit).
+//     The warps after them are TMA producers.
 //   * PERSISTENT: the grid is (#SMs x CTAs/SM); a CTA draws every tile, the first one included, from a global
-//     ticket counter (N tile fastest, so neighbouring CTAs share the A tile in L2); warp 0 publishes every tile index to
-//     the MMA and epilogue warps through a small mbarrier-guarded ring in shared memory.  The operand ring (full/empty mbarriers,
-//     tcgen05.commit releases a stage) keeps running across tile boundaries, and the accumulator is
-//     double-buffered in TMEM (tmem_full / tmem_empty barriers): while the epilogue warps drain tile i, the MMA
-//     warp is already accumulating tile i+1 and the producer is loading tile i+2.  (The first version launched
-//     one CTA per tile: 25 600 CTAs for the stem, tensor pipe 6 % active -- profiles/.)
+//     ticket counter (N tile fastest, so neighbouring CTAs share the A tile in L2); the first producer warp publishes every tile
+//     index to the other warps through a small mbarrier-guarded ring in shared memory.  The operand ring (full/empty mbarriers)
+//     keeps running across tile boundaries: the producers load the next tile's operands while the consumers run the epilogue.
 //   * HALO mode (3x3, stride 1): one (TH+2) x (TW+2) input tile per K chunk instead of one tile per tap; the nine taps
 //     are shifted windows of it (descriptor start + (kh*(TW+2) + kw) * BK*2 B, 8-row groups strided by the halo row pitch; BK = 16 / 32 use the 32- / 64-byte swizzle the same way).
 //   * ROW-PACKED stem (Cin = 16): the three kw taps of a kernel row form one 64-wide K chunk through an
@@ -44,14 +41,15 @@
 #include <cstdio>
 #include <cstdlib>
 #include "../../include/b200track.h"
+#include "b2t_wgmma.cuh"
 
 namespace {
 
 constexpr int kMaxStages = 8;
-constexpr int kTileM = 128;        // pixels per sub-tile = rows of one tcgen05.mma
+constexpr int kTileM = 128;        // pixels per sub-tile = rows of two m64 wgmma warpgroups
 constexpr int kMaxHalo = 3;        // halo-tile buffers (halo mode)
 constexpr int kRing = 4;           // tile-index ring depth (the producer runs at most a few tiles ahead)
-constexpr int kMaxProducers = 2;   // warps [0, P) = TMA producers, warp P = MMA issuer, then 4 epilogue warps per sub-tile
+constexpr int kMaxProducers = 2;   // warps [8 MT, 8 MT + P) = TMA producers after the 8 consumer warps per sub-tile
 
 struct ConvParams {
     int N, H, W, Cin;              // input geometry (Cin = channels of the slice read)
@@ -65,11 +63,11 @@ struct ConvParams {
     int tps;                       // halo mode: filter taps per weight-ring stage: 1, 3 (one kernel row = ONE 3-D TMA box) or 9 (b_res)
     int b_res;                     // halo mode, one K chunk, one N tile: the CTA's nine weight tiles are loaded once and stay resident
     int out_bufs;                  // epilogue staging boxes (128 pixels x 128 B each) per sub-tile: 1 or 2
-    int MT;                        // sub-tiles of 128 pixels per tile (1 or 2): every weight tile that reaches shared memory feeds MT MMAs
+    int MT;                        // sub-tiles of 128 pixels per tile (1 or 2): every weight tile that reaches shared memory feeds MT sub-tiles
     int sub_off;                   // bytes from sub-tile 0's A operand to sub-tile 1's inside a stage / halo buffer
     int TH, TW;                    // spatial extent of ONE sub-tile, TH*TW == 128
     int BK;                        // K chunk: 64 (SW128), 32 (SW64) or 16 (SW32) channels
-    int BN;                        // output channels per CTA, multiple of 16, <= 256
+    int BN;                        // output channels per CTA: 32, 64, 128 or 256 (the wgmma N)
     int tiles_w, tiles_h;          // tiles per image
     int out_pitch;                 // elements per output pixel (concat buffer width)
     int out_coff;                  // channel offset inside the output buffer
@@ -80,17 +78,14 @@ struct ConvParams {
     int f16;                       // 1 = operands (and 16-bit outputs) are IEEE fp16, 0 = bf16
     int flat;                      // 1 = 1x1/s1: pixels are the flattened N*H*W axis (2-D A map), TH/TW unused
     int stages;                    // shared-memory ring depth (<= kMaxStages)
-    int tmem_cols;                 // power of two >= 2 * MT * acc_cols
-    int acc_cols;                  // TMEM columns of one accumulator (BN rounded up to 32)
     int tiles_m, tiles_n;          // tile grid; tile t -> (m = t / tiles_n, n = t % tiles_n)
-    int P;                         // TMA producer warps (1..4): a thread's bulk-tensor copies are served one after the other (~470 clk per
-                                   // box whatever its size, profiles/r02_probe_tma_producers.log), so ONE producer cannot feed a CTA that runs alone on its SM
+    int P;                         // TMA producer warps (1..2): a thread's bulk-tensor copies are served one after the other,
+                                   // so two issuing threads fill the ring faster than one
     int splits;                    // split-K: work unit u = tile * splits + split; partial sums meet in `ws`
     int ksteps;                    // K steps of a whole tile: halo mode = channel chunks (9 taps each), otherwise taps x chunks
     long long total_pix;           // N*Ho*Wo (flat mode bound)
     float* ws;                     // split-K workspace [unit][MT][128][BN] fp32 (splits > 1)
     int* flags;                    // split-K arrival counters [tile][MT], self-resetting
-    long long* trace;              // B2T_CONV_TRACE builds: per-CTA cycle counters (tools/conv_trace.py), else unused
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -100,6 +95,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     asm volatile(
@@ -133,52 +131,23 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void*
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                  ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
 // one lane of a converged warp (elect.sync): the caller's control flow stays uniform up to this branch
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
     return pred != 0;
 }
-// D[tmem] (+)= A[smem] * B[smem]; descriptors passed as (lo, hi) words
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-        ::"r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate) : "memory");
-}
-// K-major operand tile: rows of (BK*2) bytes, 8-row swizzle atoms stacked every 8*(BK*2) bytes.
-// sbo_bytes = distance between consecutive 8-row groups.  The hardware applies the swizzle to the absolute shared-memory
-// address (measured: tools/probe/probe_desc.cu, profiles/r01_probe_smem_desc_shift.log), so the start address may be
-// shifted by whole 128-byte rows and sbo_bytes may be any multiple of 128 -- what the halo-tile windows rely on.
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, int row_bytes, int sbo_bytes = 0) {
-    const uint32_t sbo = (uint32_t)(sbo_bytes > 0 ? sbo_bytes : 8 * row_bytes) >> 4;
-    const uint32_t layout = row_bytes == 128 ? 2u : (row_bytes == 64 ? 4u : 6u);     // SWIZZLE_128B / 64B / 32B
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3fff);
-    d |= (uint64_t)1 << 16;                 // leading byte offset (unused for swizzled K-major), 16-byte units
-    d |= (uint64_t)(sbo & 0x3fff) << 32;    // stride byte offset
-    d |= (uint64_t)1 << 46;                 // descriptor version (Blackwell)
-    d |= (uint64_t)layout << 61;
-    return d;
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across wgmma fences / waits
+template <int R> __device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 // SiLU with ONE SFU operation: x * sigmoid(x) = h + h * tanh(h), h = x / 2  (MUFU.TANH + 1 FMUL + 1 FFMA per element).
-// Measured on the B200 (tools/probe/probe_bw.cu, profiles/r02_probe_bw.log): 27.8 elements / clk / SM against 12.8 for the
-// ex2 + rcp form this replaces, max |error| 1.0e-5 on [-12, 12] -- below fp16 output rounding for |x| > 0.02 and far below
-// bf16's.  The epilogue's SFU time for the 1.76 G activations of a batch-8 step drops from 0.47 ms to 0.22 ms of SM time.
+// max |error| 1.0e-5 on [-12, 12] -- below fp16 output rounding for |x| > 0.02 and far below bf16's.
 __device__ __forceinline__ float silu(float v) {
     const float h = 0.5f * v;
     float t;
@@ -186,149 +155,113 @@ __device__ __forceinline__ float silu(float v) {
     return fmaf(h, t, h);
 }
 
-#define B2T_TMEM_LD32(v, addr)                                                                                                     \
-    asm volatile(                                                                                                                  \
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "                                                                                  \
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                                  \
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"                                  \
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),  \
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),     \
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),     \
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])                                                                       \
-        : "r"(addr))
-
 __device__ __forceinline__ uint32_t pack16(float a, float b, bool f16) {
     if (f16) { const __half2 h = __floats2half2_rn(a, b); return *reinterpret_cast<const uint32_t*>(&h); }
     const __nv_bfloat162 h = __floats2bfloat162_rn(a, b); return *reinterpret_cast<const uint32_t*>(&h);
 }
 
-
-// One 32-column block of the accumulator row owned by this thread: + bias (padded array, float4 loads) -> SiLU ->
-// 16-bit / fp32 -> 16-byte chunks of the 128-byte-swizzled staging row.
-template <bool ACT, bool F32, bool F16>
-__device__ __forceinline__ void epilogue_block(const uint32_t (&v)[32], const float* __restrict__ bias_c, uint8_t* rowp, int chunk0, int row, float floor_v, float slope_v) {
-    const float4* b4 = reinterpret_cast<const float4*>(bias_c);
-    if (F32) {
+// Staging box bx (128 pixel rows x 128 bytes = 64 halves / 32 floats of channels, 128-byte swizzle) of one sub-tile, the part this
+// thread holds: wgmma's m64 fragment gives thread (warp w, lane l) of a warpgroup rows 16 w + l / 4 and + 8, and in every group of 8
+// columns the two at 2 (l % 4).  r0 = the first of its two rows inside the sub-tile.  + bias -> activation -> 16-bit / fp32.
+// (The column groups are walked at compile time and filtered by the box index, so the accumulator stays in registers.)
+template <bool F32, bool F16, int BN>
+__device__ __forceinline__ void stage_box(const float (&acc)[BN / 2], int bx, const float* __restrict__ bias_c, uint8_t* box, int r0, int lane,
+                                          int act, float floor_v, float slope_v) {
+    constexpr int cpb = F32 ? 32 : 64;
+    const int cq = 2 * (lane & 3);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {                 // 32 floats = one full 128-byte row
-            const float4 b = __ldg(b4 + j);
-            float4 o;
-            o.x = __uint_as_float(v[4 * j]) + b.x; o.y = __uint_as_float(v[4 * j + 1]) + b.y;
-            o.z = __uint_as_float(v[4 * j + 2]) + b.z; o.w = __uint_as_float(v[4 * j + 3]) + b.w;
-            if (ACT) { o.x = silu(o.x); o.y = silu(o.y); o.z = silu(o.z); o.w = silu(o.w); }
+    for (int j = 0; j < BN / 8; ++j) {
+        if ((8 * j) / cpb != bx) continue;
+        const int col = 8 * j + cq;
+        const float2 b = __ldg(reinterpret_cast<const float2*>(bias_c + col));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int r = r0 + 8 * h;
+            float v0 = acc[4 * j + 2 * h] + b.x, v1 = acc[4 * j + 2 * h + 1] + b.y;
+            if (act) { v0 = silu(v0); v1 = silu(v1); }
             else {        // linear: floor -inf, slope 1 (max(v, v)); ReLU: floor 0, slope 1; LeakyReLU(a): floor -inf, slope a
-                o.x = fmaxf(fmaxf(o.x, floor_v), o.x * slope_v); o.y = fmaxf(fmaxf(o.y, floor_v), o.y * slope_v);
-                o.z = fmaxf(fmaxf(o.z, floor_v), o.z * slope_v); o.w = fmaxf(fmaxf(o.w, floor_v), o.w * slope_v);
+                v0 = fmaxf(fmaxf(v0, floor_v), v0 * slope_v); v1 = fmaxf(fmaxf(v1, floor_v), v1 * slope_v);
             }
-            *reinterpret_cast<float4*>(rowp + ((j ^ (row & 7)) << 4)) = o;
-        }
-    } else {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {                 // 32 halves = 4 of the row's 8 chunks
-            const float4 b0 = __ldg(b4 + 2 * j), b1 = __ldg(b4 + 2 * j + 1);
-            float f0 = __uint_as_float(v[8 * j]) + b0.x, f1 = __uint_as_float(v[8 * j + 1]) + b0.y;
-            float f2 = __uint_as_float(v[8 * j + 2]) + b0.z, f3 = __uint_as_float(v[8 * j + 3]) + b0.w;
-            float f4 = __uint_as_float(v[8 * j + 4]) + b1.x, f5 = __uint_as_float(v[8 * j + 5]) + b1.y;
-            float f6 = __uint_as_float(v[8 * j + 6]) + b1.z, f7 = __uint_as_float(v[8 * j + 7]) + b1.w;
-            if (ACT) { f0 = silu(f0); f1 = silu(f1); f2 = silu(f2); f3 = silu(f3); f4 = silu(f4); f5 = silu(f5); f6 = silu(f6); f7 = silu(f7); }
-            else {
-                f0 = fmaxf(fmaxf(f0, floor_v), f0 * slope_v); f1 = fmaxf(fmaxf(f1, floor_v), f1 * slope_v); f2 = fmaxf(fmaxf(f2, floor_v), f2 * slope_v);
-                f3 = fmaxf(fmaxf(f3, floor_v), f3 * slope_v); f4 = fmaxf(fmaxf(f4, floor_v), f4 * slope_v); f5 = fmaxf(fmaxf(f5, floor_v), f5 * slope_v);
-                f6 = fmaxf(fmaxf(f6, floor_v), f6 * slope_v); f7 = fmaxf(fmaxf(f7, floor_v), f7 * slope_v);
-            }
-            uint4 u;
-            u.x = pack16(f0, f1, F16); u.y = pack16(f2, f3, F16); u.z = pack16(f4, f5, F16); u.w = pack16(f6, f7, F16);
-            *reinterpret_cast<uint4*>(rowp + (((chunk0 + j) ^ (row & 7)) << 4)) = u;
+            const int byte = (col - bx * cpb) * (F32 ? 4 : 2);
+            uint8_t* dst = box + r * 128 + ((((byte >> 4) ^ (r & 7)) << 4) | (byte & 15));
+            if (F32) *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+            else *reinterpret_cast<uint32_t*>(dst) = pack16(v0, v1, F16);
         }
     }
 }
 
-template <bool ACT, bool F32, bool F16, int MT, bool SPLIT>
-__global__ void __launch_bounds__(32 * (kMaxProducers + 1) + 128 * MT, MT == 1 ? 2 : 1)
+template <bool F32, bool F16, int MT, int BN>
+__global__ void __launch_bounds__(256 * MT + 32 * kMaxProducers, (MT == 1 && BN <= 64) ? 2 : 1)
 conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                      const __grid_constant__ CUtensorMap map_c, const float* __restrict__ bias, int* __restrict__ sched,
                      const ConvParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
+    constexpr int kConsumerWarps = 8 * MT;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int a_bytes = kTileM * p.BK * 2;             // one sub-tile's A operand (generic / flat mode)
-    const int b_bytes = p.BN * p.BK * 2;
+    const int b_bytes = BN * p.BK * 2;
     // generic mode: a ring of (MT A sub-tiles + B tile) stages.  halo mode: p.halo_bufs halo tiles, then a ring of B tiles.
     const int stage_bytes = (((p.halo ? p.tps * b_bytes : (MT * a_bytes + b_bytes) * p.kpair) + 1023) / 1024) * 1024;
     // swizzled operand tiles need 1024-byte alignment in the shared window (slack is reserved by the host)
     uint8_t* tiles = smem + ((1024u - (smem_u32(smem) & 1023u)) & 1023u);
     uint8_t* ring = tiles + (p.halo ? p.halo_bufs * p.halo_bytes : 0);
     const int kStages = p.stages;
-    constexpr int esize = F32 ? 4 : 2;
     constexpr int box_bytes = kTileM * 128;             // one staging box: 128 pixels x 128 B (64 halves / 32 floats of channels)
-    const int staging_bytes = p.out_bufs * box_bytes;   // per epilogue group (sub-tile)
+    const int staging_bytes = p.out_bufs * box_bytes;   // per sub-tile
     uint8_t* stage_out = ring + kStages * stage_bytes;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(stage_out + MT * staging_bytes);
     uint64_t* empty_bar = full_bar + kMaxStages;
-    uint64_t* tmem_full = empty_bar + kMaxStages;                             // [2]
-    uint64_t* tmem_empty = tmem_full + 2;                                     // [2]
-    uint64_t* ring_full = tmem_empty + 2;                                     // [kRing] tile-index ring, producer -> MMA + epilogue
+    uint64_t* ring_full = empty_bar + kMaxStages;                             // [kRing] tile-index ring, producer -> everybody else
     uint64_t* ring_empty = ring_full + kRing;                                 // [kRing]
     uint64_t* a_full = ring_empty + kRing;                                    // [kMaxHalo] halo-tile ring (halo mode)
     uint64_t* a_empty = a_full + kMaxHalo;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(a_empty + kMaxHalo);
-    int* tile_ring = reinterpret_cast<int*>(tmem_slot + 1);                   // [kRing]
-    int* last_flag = tile_ring + kRing;                                       // [2] split-K: "this group reduces the tile"
+    int* tile_ring = reinterpret_cast<int*>(a_empty + kMaxHalo);              // [kRing]
+    int* last_flag = tile_ring + kRing;                                       // [2] split-K: "this sub-tile's group reduces the tile"
     int* first_unit = last_flag + 2;                                          // the CTA's first work unit (ticket drawn at entry)
 
-    const int kchunks = p.Cin / p.BK;
+    // generic mode walks K channel-chunk-major (step kt = chunk kt / taps, tap kt % taps), the order the halo mode accumulates in:
+    // every addressing variant of a layer sums each output in the same order, so the autotuner's choice cannot change a result bit
+    const int ntaps = p.KH * p.KW;
     const int total_units = p.tiles_m * p.tiles_n * p.splits;
+    const int P = p.P;
+    const int pw = warp - kConsumerWarps;               // producer warp index (< 0: consumer)
 
     // Programmatic dependent launch: let the next layer's CTAs be scheduled as soon as every CTA of this grid is running;
-    // they do their own setup (barriers, TMEM, descriptor prefetch) in the shadow of this layer's tail and then block in
+    // they do their own setup (barriers, descriptor prefetch) in the shadow of this layer's tail and then block in
     // griddepcontrol.wait below until this grid has completed.  (No-ops when launched without the attribute.)
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     // EVERY work unit is a ticket, the first one included: a CTA that becomes resident late (another stream's kernel -- the tracker
     // step of the previous frame -- holds its SM) draws a ticket past the end and retires at once instead of owning a tile that
     // would then run after everybody else has finished.  The launch's counter pair is one of four rotating sets (b2t_conv_run), so
     // drawing before griddepcontrol.wait cannot meet the previous launch of the same plan.  The atomic's latency hides behind the setup.
-    int ticket0 = 0;
-    if (warp == 0 && lane == 0) ticket0 = atomicAdd(sched, 1);
-    // ---- one-time setup
-    if (warp == 0 && lane == 0) {
+    if (pw == 0 && lane == 0) {
+        *first_unit = atomicAdd(sched, 1);
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_c) : "memory");
-    }
-    const int P = p.P;
-    if (warp == P && lane == 0) {
-        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&tmem_full[b], 1); mbar_init(&tmem_empty[b], 4 * MT); }
-        for (int r = 0; r < kRing; ++r) { mbar_init(&ring_full[r], 1); mbar_init(&ring_empty[r], P + 4 * MT); }     // readers: the other producers + MMA + epilogue warps
-        for (int h = 0; h < kMaxHalo; ++h) { mbar_init(&a_full[h], 1); mbar_init(&a_empty[h], 1); }
+        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2 * MT); }   // released by every consumer warpgroup
+        for (int r = 0; r < kRing; ++r) { mbar_init(&ring_full[r], 1); mbar_init(&ring_empty[r], P - 1 + kConsumerWarps); }
+        for (int h = 0; h < kMaxHalo; ++h) { mbar_init(&a_full[h], 1); mbar_init(&a_empty[h], 2 * MT); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    __syncwarp();
-    if (warp == P) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (warp == 0 && lane == 0) *first_unit = ticket0;
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     // griddepcontrol.wait (the previous kernel in the stream has completed, its writes are visible) is executed by the producer
     // warps only, AFTER they have requested the first weight tiles: weights do not depend on the previous layer, so their DRAM
     // latency and the first ring fill overlap its tail.  Every other global access of this kernel is ordered after a producer's
-    // loads through the mbarrier chain (activation tiles -> MMAs -> accumulators -> epilogue stores, split-K workspace, tickets).
+    // loads through the mbarrier chain (activation tiles -> MMAs -> epilogue stores, split-K workspace, tickets).
 
     // work unit u -> tile coordinates and K-step range [k0, k1)
     auto unit_coords = [&](int u, int& n0, int& img, int& ho0, int& wo0, long long& pix0, int& k0, int& k1) {
         int t = u;
         k0 = 0; k1 = p.ksteps;
-        if (SPLIT) {
+        if (p.splits > 1) {
             t = u / p.splits;
             const int sp = u - t * p.splits;
             k0 = (p.ksteps * sp) / p.splits;
             k1 = (p.ksteps * (sp + 1)) / p.splits;
         }
         const int mt = t / p.tiles_n, nt = t % p.tiles_n;
-        n0 = nt * p.BN; img = 0; ho0 = 0; wo0 = 0; pix0 = 0;
+        n0 = nt * BN; img = 0; ho0 = 0; wo0 = 0; pix0 = 0;
         if (p.flat) pix0 = (long long)mt * (kTileM * MT);
         else {
             const int per_img = p.tiles_w * p.tiles_h;
@@ -340,324 +273,280 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
         }
     };
 
-    if (warp < P) {
-        // ===== TMA producers.  Warp 0 is also the tile scheduler: the first unit is the ticket drawn at entry, later ones are drawn from the same
-        // global counter, so a CTA that starts late (or shares its SM with another stream's kernel) simply takes fewer tiles
-        // instead of stretching the layer; every unit index (and the final -1) is published to the other producers, the MMA
-        // and the epilogue warps through a small shared-memory ring.  The K steps of the operand ring are dealt round-robin
+    if (pw >= 0) {
+        // ===== TMA producers.  Producer 0 is also the tile scheduler: the first unit is the ticket drawn at entry, later ones are drawn from
+        // the same global counter, so a CTA that starts late (or shares its SM with another stream's kernel) simply takes fewer tiles
+        // instead of stretching the layer; every unit index (and the final -1) is published to the other producer and the consumer
+        // warps through a small shared-memory ring.  The K steps of the operand ring are dealt round-robin
         // to the P producers (step c belongs to producer c % P): bulk-tensor copies issued by one thread are served one at a
-        // time, so P issuing threads give P times the fill rate.  All producers run ahead of the MMA warp, across tile boundaries.
-        // (whole warp, uniform control flow; one elected lane issues the copies -- see the MMA warp below)
-        {
-            int stage = 0; uint32_t phase = 0;
-            int hbuf = 0; uint32_t hphase = 0;
-            int rslot = 0; uint32_t rphase = 0;
-            int c = 0;                                  // operand-ring step counter: (c % P == warp) -> this producer loads it
-            int u = *first_unit;
-            // weight tile(s) of ring step `s` of a unit that starts at K step k0 (n0 = its first output channel)
-            const int groups = p.halo ? 9 / p.tps : 1;         // halo mode: weight boxes per K chunk
-            auto load_b = [&](int st, int n0, int k0, int s) {
-                uint8_t* sb = ring + st * stage_bytes + (p.halo ? 0 : MT * a_bytes * p.kpair);
-                if (p.halo) {
-                    const int kc = k0 + s / groups, tap = (s % groups) * p.tps;
-                    if (p.tps == 1) tma_load_2d(sb, &map_b, &full_bar[st], tap * p.Cin + kc * p.BK, n0);
-                    else tma_load_3d(sb, &map_b, &full_bar[st], kc * p.BK, n0, tap);     // one kernel row: taps tap .. tap + 2
-                } else if (p.kpair == 2) {
-                    tma_load_3d(sb, &map_b, &full_bar[st], 0, n0, 2 * (k0 + s));
-                } else {
-                    const int kt = k0 + s, tap = kt / kchunks, kc = kt % kchunks;
-                    tma_load_2d(sb, &map_b, &full_bar[st], tap * p.Cin + kc * p.BK, n0);
-                }
-            };
-            const uint32_t stage_tx = (uint32_t)(p.halo ? p.tps * b_bytes : (MT * a_bytes + b_bytes) * p.kpair);
-            int npre = 0;                               // ring steps of the FIRST unit whose weights were requested before the wait
-            if (u < total_units) {
-                int n0, img, ho0, wo0, k0, k1; long long pix0;
-                unit_coords(u, n0, img, ho0, wo0, pix0, k0, k1);
-                if (p.b_res) {
-                    if (warp == 0 && elect_one()) {
-                        mbar_expect_tx(&full_bar[0], (uint32_t)(9 * b_bytes));
-                        tma_load_3d(ring, &map_b, &full_bar[0], 0, n0, 0);
-                    }
-                } else {
-                    const int nsteps = (k1 - k0) * groups;
-                    npre = nsteps < kStages ? nsteps : kStages;
-                    for (int s = warp; s < npre; s += P)
-                        if (elect_one()) {
-                            mbar_expect_tx(&full_bar[s], stage_tx);
-                            load_b(s, n0, k0, s);
-                        }
-                }
-                __syncwarp();
-            }
-            asm volatile("griddepcontrol.wait;" ::: "memory");
-            for (;;) {
-                if (warp == 0) {
-                    const bool live = u < total_units;
-                    mbar_wait(&ring_empty[rslot], rphase ^ 1);
-                    if (lane == 0) {
-                        tile_ring[rslot] = live ? u : -1;
-                        asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&ring_full[rslot])) : "memory");
-                    }
-                    __syncwarp();
-                    if (++rslot == kRing) { rslot = 0; rphase ^= 1; }
-                    if (!live) break;
-                } else {
-                    mbar_wait(&ring_full[rslot], rphase);
-                    u = tile_ring[rslot];
-                    __syncwarp();
-                    if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&ring_empty[rslot])) : "memory");
-                    if (++rslot == kRing) { rslot = 0; rphase ^= 1; }
-                    if (u < 0) break;
-                }
-                // next unit: latency hidden behind this unit's loads
-                int next = 0;
-                if (warp == 0) {
-                    if (lane == 0) next = atomicAdd(sched, 1);
-                    next = __shfl_sync(0xffffffffu, next, 0);
-                }
-                int n0, img, ho0, wo0, k0, k1; long long pix0;
-                unit_coords(u, n0, img, ho0, wo0, pix0, k0, k1);
-                if (p.halo) {
-                    // one (TH+2) x (MT*TW+2) x 64-channel input tile per K chunk (zero-filled outside the image = the padding),
-                    // then the nine taps' weight tiles through the B ring
-                    const uint32_t halo_tx = (uint32_t)((p.TW * MT + 2) * (p.TH + 2) * p.BK * 2);
-                    auto load_halo = [&](int kc) {              // producer 0 only
-                        mbar_wait(&a_empty[hbuf], hphase ^ 1);
-                        if (elect_one()) {
-                            mbar_expect_tx(&a_full[hbuf], halo_tx);
-                            tma_load_4d(tiles + hbuf * p.halo_bytes, &map_a, &a_full[hbuf], kc * p.BK, wo0 - 1, ho0 - 1, img);
-                        }
-                        __syncwarp();
-                        if (++hbuf == p.halo_bufs) { hbuf = 0; hphase ^= 1; }
-                    };
-                    // the input tile of chunk kc + 1 is requested BEFORE the weight tiles of chunk kc: the producer blocks on
-                    // the weight ring long before the MMA warp is done with chunk kc, and a late halo tile stalls nine taps
-                    if (warp == 0) load_halo(k0);
-                    for (int kc = k0; kc < k1; ++kc) {
-                        if (warp == 0 && kc + 1 < k1) load_halo(kc + 1);
-                        if (p.b_res) continue;        // the whole weight slice (nine taps of the single K chunk) landed once, before the wait
-                        for (int g = 0; g < groups; ++g, ++c) {
-                            if (c % P == warp && c >= npre) {      // (the first npre steps were requested before griddepcontrol.wait)
-                                mbar_wait(&empty_bar[stage], phase ^ 1);
-                                if (elect_one()) {
-                                    mbar_expect_tx(&full_bar[stage], stage_tx);
-                                    load_b(stage, n0, kc, g);
-                                }
-                                __syncwarp();
-                            }
-                            if (++stage == kStages) { stage = 0; phase ^= 1; }
-                        }
-                    }
-                } else
-                for (int kt = k0; kt < k1; ++kt, ++c) {
-                    if (c % P == warp) {
-                        const int tap = kt / kchunks, kc = kt % kchunks;
-                        const int kh = tap / p.KW, kw = tap % p.KW;
-                        const bool pre = c < npre;         // weights (and the byte count) of this step went out before the wait
-                        mbar_wait(&empty_bar[stage], phase ^ 1);
-                        if (elect_one()) {
-                            uint8_t* sa = ring + stage * stage_bytes;
-                            if (!pre) mbar_expect_tx(&full_bar[stage], stage_tx);
-                            if (p.kpair == 2) tma_load_3d(sa, &map_a, &full_bar[stage], 0, (int)pix0, 2 * kt);      // chunks 2 kt, 2 kt + 1: one {64, rows, 2} box
-                            else if (p.flat) tma_load_2d(sa, &map_a, &full_bar[stage], kc * p.BK, (int)pix0);
-                            else tma_load_4d(sa, &map_a, &full_bar[stage], kc * p.BK, wo0 * p.stride + kw - p.pad_w, ho0 * p.stride + kh - p.pad, img);
-                            if (!pre) load_b(stage, n0, kt, 0);
-                        }
-                        __syncwarp();
-                    }
-                    if (++stage == kStages) { stage = 0; phase ^= 1; }
-                }
-                u = next;
-            }
-            // every CTA draws exactly one ticket past the end; the last one to do so re-arms the counters for the next launch
-            if (warp == 0 && lane == 0 && atomicAdd(sched + 1, 1) == (int)gridDim.x - 1) {
-                sched[0] = 0; sched[1] = 0;
-                __threadfence();
-            }
-        }
-    } else if (warp == P) {
-        // ===== MMA issuer: accumulator set (i & 1) = MT accumulators, released by the epilogue groups through tmem_empty.
-        // The WHOLE warp runs this loop (uniform control flow: descriptors live in uniform registers) and one elected lane issues
-        // the tcgen05 instructions.  Running it under `if (lane == 0)` made ptxas wrap every UTCHMMA in a lane-uniformity
-        // ("waterfall") loop -- ~16 issue slots per MMA, ~190 per tap -- and the issuing thread, not the tensor pipe or the
-        // operand ring, bounded every layer (profiles/r02_conv_mma_issue_bound_sass_samples.csv: the ring was never empty).
-        // instruction descriptor: D = fp32 (bits 4-5), A / B format (bits 7-9 / 10-12: 0 = fp16, 1 = bf16), N >> 3, M >> 4
-        const uint32_t idesc = (1u << 4) | (F16 ? 0u : ((1u << 7) | (1u << 10))) | ((uint32_t)(p.BN >> 3) << 17) | ((uint32_t)(kTileM >> 4) << 24);
-        const int row_bytes = p.BK * 2;
-        const int halo_w = p.TW * MT + 2;
-        // shared-memory descriptor = {lo: (address >> 4) | LBO 1 << 16, hi: SBO >> 4 | version 1 << 14 | swizzle mode << 29}
-        const uint32_t layout = row_bytes == 128 ? 2u : (row_bytes == 64 ? 4u : 6u);
-        const uint32_t hi_b = (uint32_t)((8 * row_bytes) >> 4) | (1u << 14) | (layout << 29);
-        const uint32_t hi_a = p.halo ? ((uint32_t)((halo_w * row_bytes) >> 4) | (1u << 14) | (layout << 29)) : hi_b;
-        const uint32_t ring_lo = ((smem_u32(ring) >> 4) & 0x3fffu) | (1u << 16);
-        const uint32_t tiles_lo = ((smem_u32(tiles) >> 4) & 0x3fffu) | (1u << 16);
-        const uint32_t stage_step = (uint32_t)stage_bytes >> 4, halo_step = (uint32_t)p.halo_bytes >> 4;
-        const uint32_t sub_step = (uint32_t)p.sub_off >> 4, b_off = (uint32_t)(MT * a_bytes) >> 4, b_step = (uint32_t)b_bytes >> 4;
-        bool b_ready = false;
-        const int ksub = p.BK / 16;
-        const uint32_t row_step = (uint32_t)row_bytes >> 4;        // halo windows shift by whole pixel rows of the tile
+        // time, so P issuing threads give P times the fill rate.  All producers run ahead of the consumers, across tile boundaries.
+        // (whole warp, uniform control flow; one elected lane issues the copies)
         int stage = 0; uint32_t phase = 0;
         int hbuf = 0; uint32_t hphase = 0;
         int rslot = 0; uint32_t rphase = 0;
-#ifdef B2T_CONV_TRACE
-        long long t_ring = 0, t_tmem = 0, t_afull = 0, t_full = 0, t_issue = 0, t_tot = clock64(), tt;
-#define TR_BEGIN() tt = clock64()
-#define TR_END(acc) acc += clock64() - tt
-#else
-#define TR_BEGIN()
-#define TR_END(acc)
-#endif
-        for (int i = 0;; ++i) {
-            TR_BEGIN();
+        int c = 0;                                  // operand-ring step counter: (c % P == pw) -> this producer loads it
+        int u = *first_unit;
+        // weight tile(s) of ring step `s` of a unit that starts at K step k0 (n0 = its first output channel)
+        const int groups = p.halo ? 9 / p.tps : 1;         // halo mode: weight boxes per K chunk
+        auto load_b = [&](int st, int n0, int k0, int s) {
+            uint8_t* sb = ring + st * stage_bytes + (p.halo ? 0 : MT * a_bytes * p.kpair);
+            if (p.halo) {
+                const int kc = k0 + s / groups, tap = (s % groups) * p.tps;
+                if (p.tps == 1) tma_load_2d(sb, &map_b, &full_bar[st], tap * p.Cin + kc * p.BK, n0);
+                else tma_load_3d(sb, &map_b, &full_bar[st], kc * p.BK, n0, tap);     // one kernel row: taps tap .. tap + 2
+            } else if (p.kpair == 2) {
+                tma_load_3d(sb, &map_b, &full_bar[st], 0, n0, 2 * (k0 + s));
+            } else {
+                const int kt = k0 + s, kc = kt / ntaps, tap = kt % ntaps;
+                tma_load_2d(sb, &map_b, &full_bar[st], tap * p.Cin + kc * p.BK, n0);
+            }
+        };
+        const uint32_t stage_tx = (uint32_t)(p.halo ? p.tps * b_bytes : (MT * a_bytes + b_bytes) * p.kpair);
+        int npre = 0;                               // ring steps of the FIRST unit whose weights were requested before the wait
+        if (u < total_units) {
+            int n0, img, ho0, wo0, k0, k1; long long pix0;
+            unit_coords(u, n0, img, ho0, wo0, pix0, k0, k1);
+            if (p.b_res) {
+                if (pw == 0 && elect_one()) {
+                    mbar_expect_tx(&full_bar[0], (uint32_t)(9 * b_bytes));
+                    tma_load_3d(ring, &map_b, &full_bar[0], 0, n0, 0);
+                }
+            } else {
+                const int nsteps = (k1 - k0) * groups;
+                npre = nsteps < kStages ? nsteps : kStages;
+                for (int s = pw; s < npre; s += P)
+                    if (elect_one()) {
+                        mbar_expect_tx(&full_bar[s], stage_tx);
+                        load_b(s, n0, k0, s);
+                    }
+            }
+            __syncwarp();
+        }
+        asm volatile("griddepcontrol.wait;" ::: "memory");
+        for (;;) {
+            if (pw == 0) {
+                const bool live = u < total_units;
+                mbar_wait(&ring_empty[rslot], rphase ^ 1);
+                if (lane == 0) {
+                    tile_ring[rslot] = live ? u : -1;
+                    mbar_arrive(&ring_full[rslot]);
+                }
+                __syncwarp();
+                if (++rslot == kRing) { rslot = 0; rphase ^= 1; }
+                if (!live) break;
+            } else {
+                mbar_wait(&ring_full[rslot], rphase);
+                u = tile_ring[rslot];
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&ring_empty[rslot]);
+                if (++rslot == kRing) { rslot = 0; rphase ^= 1; }
+                if (u < 0) break;
+            }
+            // next unit: latency hidden behind this unit's loads
+            int next = 0;
+            if (pw == 0) {
+                if (lane == 0) next = atomicAdd(sched, 1);
+                next = __shfl_sync(0xffffffffu, next, 0);
+            }
+            int n0, img, ho0, wo0, k0, k1; long long pix0;
+            unit_coords(u, n0, img, ho0, wo0, pix0, k0, k1);
+            if (p.halo) {
+                // one (TH+2) x (MT*TW+2) x BK-channel input tile per K chunk (zero-filled outside the image = the padding),
+                // then the nine taps' weight tiles through the B ring
+                const uint32_t halo_tx = (uint32_t)((p.TW * MT + 2) * (p.TH + 2) * p.BK * 2);
+                auto load_halo = [&](int kc) {              // producer 0 only
+                    mbar_wait(&a_empty[hbuf], hphase ^ 1);
+                    if (elect_one()) {
+                        mbar_expect_tx(&a_full[hbuf], halo_tx);
+                        tma_load_4d(tiles + hbuf * p.halo_bytes, &map_a, &a_full[hbuf], kc * p.BK, wo0 - 1, ho0 - 1, img);
+                    }
+                    __syncwarp();
+                    if (++hbuf == p.halo_bufs) { hbuf = 0; hphase ^= 1; }
+                };
+                // the input tile of chunk kc + 1 is requested BEFORE the weight tiles of chunk kc: the producer blocks on
+                // the weight ring long before the consumers are done with chunk kc, and a late halo tile stalls nine taps
+                if (pw == 0) load_halo(k0);
+                for (int kc = k0; kc < k1; ++kc) {
+                    if (pw == 0 && kc + 1 < k1) load_halo(kc + 1);
+                    if (p.b_res) continue;        // the whole weight slice (nine taps of the single K chunk) landed once, before the wait
+                    for (int g = 0; g < groups; ++g, ++c) {
+                        if (c % P == pw && c >= npre) {      // (the first npre steps were requested before griddepcontrol.wait)
+                            mbar_wait(&empty_bar[stage], phase ^ 1);
+                            if (elect_one()) {
+                                mbar_expect_tx(&full_bar[stage], stage_tx);
+                                load_b(stage, n0, kc, g);
+                            }
+                            __syncwarp();
+                        }
+                        if (++stage == kStages) { stage = 0; phase ^= 1; }
+                    }
+                }
+            } else
+            for (int kt = k0; kt < k1; ++kt, ++c) {
+                if (c % P == pw) {
+                    const int kc = kt / ntaps, tap = kt % ntaps;
+                    const int kh = tap / p.KW, kw = tap % p.KW;
+                    const bool pre = c < npre;         // weights (and the byte count) of this step went out before the wait
+                    mbar_wait(&empty_bar[stage], phase ^ 1);
+                    if (elect_one()) {
+                        uint8_t* sa = ring + stage * stage_bytes;
+                        if (!pre) mbar_expect_tx(&full_bar[stage], stage_tx);
+                        if (p.kpair == 2) tma_load_3d(sa, &map_a, &full_bar[stage], 0, (int)pix0, 2 * kt);      // chunks 2 kt, 2 kt + 1: one {64, rows, 2} box
+                        else if (p.flat) tma_load_2d(sa, &map_a, &full_bar[stage], kc * p.BK, (int)pix0);
+                        else tma_load_4d(sa, &map_a, &full_bar[stage], kc * p.BK, wo0 * p.stride + kw - p.pad_w, ho0 * p.stride + kh - p.pad, img);
+                        if (!pre) load_b(stage, n0, kt, 0);
+                    }
+                    __syncwarp();
+                }
+                if (++stage == kStages) { stage = 0; phase ^= 1; }
+            }
+            u = next;
+        }
+        // every CTA draws exactly one ticket past the end; the last one to do so re-arms the counters for the next launch
+        if (pw == 0 && lane == 0 && atomicAdd(sched + 1, 1) == (int)gridDim.x - 1) {
+            sched[0] = 0; sched[1] = 0;
+            __threadfence();
+        }
+    } else {
+        // ===== consumers: sub-tile g = warps [8 g, 8 g + 8) = two warpgroups; warpgroup half hh owns pixel rows [64 hh, 64 hh + 64) of it.
+        // Each warpgroup issues its own wgmma chain into its registers and releases a ring stage (one arrival per warpgroup) once the
+        // wgmmas that read it have retired: wait_group 1 after each stage's batch, so the tensor core always has the next batch queued.
+        const int g = warp >> 3;
+        const int hh = (warp >> 2) & 1;
+        const int gtid = (int)threadIdx.x - g * 256;      // thread index inside the sub-tile's group
+        const int bar_id = 1 + g;
+        const bool wg_leader = (threadIdx.x & 127) == 0;
+        const int r0 = hh * 64 + (warp & 3) * 16 + (lane >> 2);      // this thread's first accumulator row inside the sub-tile (and r0 + 8)
+        // shared-memory matrix descriptor = {lo: (address >> 4) | LBO 1 << 16, hi: SBO >> 4 | swizzle mode << 30 (1 = 128 B, 2 = 64 B,
+        // 3 = 32 B)}: K-major rows of BK*2 bytes, 8-row groups SBO bytes apart.  The swizzle is a function of the absolute shared-memory
+        // address (the TMA unit writes the tiles the same way), so a start address shifted by whole rows and an SBO of any multiple of
+        // the row size address a window of a larger tile -- what the halo windows rely on.  K advances by 32 bytes per k16 step.
+        const int row_bytes = p.BK * 2;
+        const int halo_w = p.TW * MT + 2;
+        const uint32_t layout = row_bytes == 128 ? 1u : (row_bytes == 64 ? 2u : 3u);
+        const uint32_t hi_b = (uint32_t)((8 * row_bytes) >> 4) | (layout << 30);
+        const uint32_t hi_a = p.halo ? ((uint32_t)((halo_w * row_bytes) >> 4) | (layout << 30)) : hi_b;
+        const uint32_t ring_lo = ((smem_u32(ring) >> 4) & 0x3fffu) | (1u << 16);
+        const uint32_t tiles_lo = ((smem_u32(tiles) >> 4) & 0x3fffu) | (1u << 16);
+        const uint32_t stage_step = (uint32_t)stage_bytes >> 4, halo_step = (uint32_t)p.halo_bytes >> 4;
+        const uint32_t b_off = (uint32_t)(MT * a_bytes) >> 4, b_step = (uint32_t)b_bytes >> 4;
+        const uint32_t row_step = (uint32_t)row_bytes >> 4;        // halo windows shift by whole pixel rows of the tile
+        // this warpgroup's 64 rows: sub-tile g (sub_off), second half = 8 row groups further (8 tile rows of the halo tile, or 64 rows)
+        const uint32_t a_off = (uint32_t)(g * p.sub_off) / 16u + (uint32_t)hh * (p.halo ? 8u * (uint32_t)halo_w * row_step : 64u * row_step);
+        auto desc = [](uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; };
+        const int ksub = p.BK / 16;
+        bool b_ready = false;
+        int stage = 0; uint32_t phase = 0;
+        int hbuf = 0; uint32_t hphase = 0;
+        int rslot = 0; uint32_t rphase = 0;
+        constexpr int cols_per_box = F32 ? 32 : 64;
+        constexpr int nboxes = (BN + cols_per_box - 1) / cols_per_box;
+        int box_seq = 0;                                  // running box counter: staging buffer = box_seq & 1 when there are two
+        float acc[BN / 2];
+        for (;;) {
             mbar_wait(&ring_full[rslot], rphase);
-            TR_END(t_ring);
             const int u = tile_ring[rslot];
             __syncwarp();
-            if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&ring_empty[rslot])) : "memory");
+            if (lane == 0) mbar_arrive(&ring_empty[rslot]);
             if (++rslot == kRing) { rslot = 0; rphase ^= 1; }
             if (u < 0) break;
             int n0, img, ho0, wo0, k0, k1; long long pix0;
             unit_coords(u, n0, img, ho0, wo0, pix0, k0, k1);
-            const int buf = i & 1;
-            TR_BEGIN();
-            mbar_wait(&tmem_empty[buf], (uint32_t)(((i >> 1) & 1) ^ 1));
-            TR_END(t_tmem);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t tacc = tmem_base + (uint32_t)(buf * MT * p.acc_cols);
-            uint32_t first = 1;                                // the first K step of the unit: each accumulator's first MMA overwrites
+            // ring stage / halo buffer read by the most recent committed batch: released once a later wait_group shows it retired
+            int pend_stage = -1, pend_halo = -1;
+            auto release = [&](int st, int hb) {
+                if (wg_leader) {
+                    if (st >= 0) mbar_arrive(&empty_bar[st]);
+                    if (hb >= 0) mbar_arrive(&a_empty[hb]);
+                }
+            };
+            // after committing a batch that read (st, hb): keep it in flight behind the next one, or -- when the producer cannot deliver the
+            // next batch's operands before these are back (a one-stage ring; the halo tile, whose successor's buffer is requested ahead of
+            // the next chunk's weights) -- wait for everything and release at once
+            auto retire = [&](int st, int hb, bool drain) {
+                if (drain) {
+                    wgmma_wait<0>();
+                    acc_fence(acc);
+                    release(pend_stage, pend_halo);
+                    release(st, hb);
+                    pend_stage = pend_halo = -1;
+                } else {
+                    wgmma_wait<1>();
+                    acc_fence(acc);
+                    release(pend_stage, pend_halo);
+                    pend_stage = st; pend_halo = hb;
+                }
+            };
+            uint32_t scale = 0;                             // the unit's first wgmma overwrites the accumulator
             if (p.halo) {
                 for (int kc = k0; kc < k1; ++kc) {
-                    TR_BEGIN();
                     mbar_wait(&a_full[hbuf], hphase);
-                    TR_END(t_afull);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t a_buf = tiles_lo + (uint32_t)hbuf * halo_step;
+                    const uint32_t a_buf = tiles_lo + (uint32_t)hbuf * halo_step + a_off;
                     for (int tap0 = 0; tap0 < 9; tap0 += p.tps) {
                         if (!p.b_res || !b_ready) {
-                            TR_BEGIN();
                             mbar_wait(&full_bar[stage], phase);
-                            TR_END(t_full);
-                            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
                             b_ready = true;
                         }
-                        TR_BEGIN();
                         const uint32_t b_stage = ring_lo + (uint32_t)stage * stage_step;
-                        if (elect_one()) {
-                            for (int t = 0; t < p.tps; ++t) {
-                                // A window of tap (kh, kw) for sub-tile s: the halo tile shifted by kh rows and kw + s*TW pixels;
-                                // the 8-row MMA groups are the tile rows, strided by the halo row pitch
-                                const int tap = tap0 + t, kh = tap / 3, kw = tap - 3 * kh;
-                                const uint32_t a_lo = a_buf + (uint32_t)(kh * halo_w + kw) * row_step;
-                                const uint32_t b_lo = b_stage + (uint32_t)t * b_step;
-#pragma unroll
-                                for (int s = 0; s < MT; ++s) {
-#pragma unroll 4
-                                    for (int k = 0; k < ksub; ++k) {
-                                        umma_f16(tacc + (uint32_t)(s * p.acc_cols), a_lo + (uint32_t)s * sub_step + 2u * k, hi_a, b_lo + 2u * k, hi_b, idesc,
-                                                 (first && t == 0 && k == 0) ? 0u : 1u);
-                                    }
-                                }
+                        acc_fence(acc);
+                        wgmma_fence();
+                        for (int t = 0; t < p.tps; ++t) {
+                            // A window of tap (kh, kw): the halo tile shifted by kh rows and kw pixels; the 8-row groups are the
+                            // tile rows, strided by the halo row pitch
+                            const int tap = tap0 + t, kh = tap / 3, kw = tap - 3 * kh;
+                            const uint32_t a_lo = a_buf + (uint32_t)(kh * halo_w + kw) * row_step;
+                            const uint32_t b_lo = b_stage + (uint32_t)t * b_step;
+                            for (int k = 0; k < ksub; ++k) {
+                                wgmma_m64k16<BN, F16>(acc, desc(a_lo + 2u * k, hi_a), desc(b_lo + 2u * k, hi_b), scale);
+                                scale = 1;
                             }
-                            if (!p.b_res) umma_commit(&empty_bar[stage]);
                         }
-                        __syncwarp();
-                        TR_END(t_issue);
-                        first = 0;
+                        wgmma_commit();
+                        const bool chunk_end = tap0 + p.tps >= 9;
+                        retire(p.b_res ? -1 : stage, chunk_end ? hbuf : -1, chunk_end || kStages == 1);
                         if (!p.b_res && ++stage == kStages) { stage = 0; phase ^= 1; }
                     }
-                    if (elect_one()) umma_commit(&a_empty[hbuf]);           // halo tile reusable once its MMAs retire
-                    __syncwarp();
                     if (++hbuf == p.halo_bufs) { hbuf = 0; hphase ^= 1; }
                 }
             } else
             for (int kt = k0; kt < k1; ++kt) {
-                TR_BEGIN();
                 mbar_wait(&full_bar[stage], phase);
-                TR_END(t_full);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                TR_BEGIN();
                 const uint32_t a_st = ring_lo + (uint32_t)stage * stage_step;
                 const uint32_t b_st = a_st + b_off * (uint32_t)p.kpair;
-                if (elect_one()) {
-                    for (int j = 0; j < p.kpair; ++j) {       // K chunks of this stage: [chunk][sub-tile][128 rows] | [chunk][BN rows]
-                        const uint32_t a_lo = a_st + (uint32_t)j * b_off, b_lo = b_st + (uint32_t)j * b_step;
-#pragma unroll
-                        for (int s = 0; s < MT; ++s)
-                            for (int k = 0; k < ksub; ++k) {
-                                umma_f16(tacc + (uint32_t)(s * p.acc_cols), a_lo + (uint32_t)s * sub_step + 2u * k, hi_a, b_lo + 2u * k, hi_b, idesc,
-                                         (first && j == 0 && k == 0) ? 0u : 1u);
-                            }
+                acc_fence(acc);
+                wgmma_fence();
+                for (int j = 0; j < p.kpair; ++j) {       // K chunks of this stage: [chunk][sub-tile][128 rows] | [chunk][BN rows]
+                    const uint32_t a_lo = a_st + (uint32_t)j * b_off + a_off, b_lo = b_st + (uint32_t)j * b_step;
+                    for (int k = 0; k < ksub; ++k) {
+                        wgmma_m64k16<BN, F16>(acc, desc(a_lo + 2u * k, hi_a), desc(b_lo + 2u * k, hi_b), scale);
+                        scale = 1;
                     }
-                    umma_commit(&empty_bar[stage]);          // stage reusable once these MMAs retire
                 }
-                __syncwarp();
-                TR_END(t_issue);
-                first = 0;
+                wgmma_commit();
+                retire(stage, -1, kStages == 1);
                 if (++stage == kStages) { stage = 0; phase ^= 1; }
             }
-            if (elect_one()) umma_commit(&tmem_full[buf]);                 // accumulators of this unit complete
-            __syncwarp();
-        }
-#ifdef B2T_CONV_TRACE
-        if (lane == 0 && p.trace) {
-            long long* tr = p.trace + (size_t)blockIdx.x * 16;
-            tr[0] = clock64() - t_tot; tr[1] = t_ring; tr[2] = t_tmem; tr[3] = t_afull; tr[4] = t_full; tr[5] = t_issue;
-        }
-#endif
-    } else {
-        // ===== epilogue: group g = sub-tile g, its four warps own TMEM lanes 32*(warp%4) .. +31 of that sub-tile's accumulator
-        const int g = (warp - P - 1) >> 2;
-        const int q = warp & 3;
-        const int row = q * 32 + lane;                    // pixel row inside the sub-tile
-        const int gtid = (int)threadIdx.x - 32 * (P + 1) - g * 128;  // thread index inside the group
-        const int bar_id = 1 + g;
-        constexpr int cols_per_box = 128 / esize;         // 64 halves or 32 floats per 128-byte staging row
-        int box_seq = 0;                                  // running box counter: staging buffer = box_seq & 1 when there are two
-        int rslot = 0; uint32_t rphase = 0;
-        for (int i = 0;; ++i) {
-            mbar_wait(&ring_full[rslot], rphase);
-            const int u = tile_ring[rslot];
-            __syncwarp();
-            if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&ring_empty[rslot])) : "memory");
-            if (++rslot == kRing) { rslot = 0; rphase ^= 1; }
-            if (u < 0) break;
-            const int buf = i & 1;
-            int n0, img, ho0, wo0, k0, k1; long long pix0;
-            unit_coords(u, n0, img, ho0, wo0, pix0, k0, k1);
+            wgmma_wait<0>();
+            acc_fence(acc);
+            release(pend_stage, pend_halo);
             // this group's output window
             const long long gpix = pix0 + (long long)g * kTileM;
             const int gho = p.halo ? ho0 : ho0 + g * p.TH;
             const int gwo = p.halo ? wo0 + g * p.TW : wo0;
             const bool in_range = p.flat ? (gpix < p.total_pix) : (gho < p.Ho && gwo < p.Wo);
-#ifdef B2T_CONV_TRACE
-            const long long e0 = clock64();
-#endif
-            mbar_wait(&tmem_full[buf], (uint32_t)((i >> 1) & 1));
-#ifdef B2T_CONV_TRACE
-            if (gtid == 0 && p.trace) { p.trace[(size_t)blockIdx.x * 16 + 8 + g * 2] += clock64() - e0; p.trace[(size_t)blockIdx.x * 16 + 9 + g * 2] += 1; }
-#endif
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)((buf * MT + g) * p.acc_cols);
             bool reduce_here = true;
-            if (SPLIT) {
+            if (p.splits > 1) {
                 // ---- split-K: park the fp32 partial sums, count arrivals; the LAST split of a tile to arrive sums all of them in
                 // split order (a fixed order: results do not depend on which CTA is last) and runs the normal epilogue
-                float* wrow = p.ws + (((size_t)u * MT + g) * kTileM + row) * p.BN;
-                for (int c0 = 0; c0 < p.BN; c0 += 32) {
-                    uint32_t v0[32];
-                    B2T_TMEM_LD32(v0, taddr + (uint32_t)c0);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+                const int cq = 2 * (lane & 3);
+                float* wsub = p.ws + ((size_t)u * MT + g) * kTileM * BN;
 #pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        __stcg(reinterpret_cast<float4*>(wrow + c0) + j, make_float4(__uint_as_float(v0[4 * j]), __uint_as_float(v0[4 * j + 1]),
-                                                                                     __uint_as_float(v0[4 * j + 2]), __uint_as_float(v0[4 * j + 3])));
-                }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&tmem_empty[buf])) : "memory");
+                for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+                        __stcg(reinterpret_cast<float2*>(wsub + (size_t)(r0 + 8 * h) * BN + 8 * j + cq), make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]));
                 __threadfence();
-                asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+                asm volatile("bar.sync %0, 256;" ::"r"(bar_id) : "memory");
                 if (gtid == 0) {
                     const int t = u / p.splits;
                     const int old = atomicAdd(p.flags + t * MT + g, 1);
@@ -665,84 +554,54 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
                     if (last) p.flags[t * MT + g] = 0;              // re-armed for the next launch
                     last_flag[g] = last;
                 }
-                asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+                asm volatile("bar.sync %0, 256;" ::"r"(bar_id) : "memory");
                 reduce_here = last_flag[g] != 0;
-                if (reduce_here) __threadfence();
-            }
-            // ---- one staging box (128 pixels x 128 B = 64 halves / 32 floats of channels) at a time: TMEM -> registers -> + bias ->
-            // SiLU -> 16-bit -> swizzled shared memory -> TMA store, the store of box b overlapping the math of box b + 1
-            const int nboxes = (p.BN + cols_per_box - 1) / cols_per_box;
-            if (reduce_here)
-            for (int bx = 0; bx < nboxes; ++bx, ++box_seq) {
-                const int c0 = bx * cols_per_box;
-                uint8_t* stage_cur = stage_out + g * staging_bytes + (p.out_bufs == 2 ? (box_seq & 1) * box_bytes : 0);
-                // the store that used this buffer (out_bufs boxes ago) must have finished READING it
-                if (gtid == 0) {
-                    if (p.out_bufs == 2) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-                    else asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                }
-                asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
-                if (in_range) {
-                    if (SPLIT) {
-                        const int t = u / p.splits;
-                        for (int cc = c0; cc < c0 + cols_per_box && cc < p.BN; cc += 32) {
-                            float acc[32];
+                if (reduce_here) {
+                    __threadfence();
+                    const int t = u / p.splits;
 #pragma unroll
-                            for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-                            for (int sp = 0; sp < p.splits; ++sp) {
-                                const float4* src = reinterpret_cast<const float4*>(p.ws + ((((size_t)t * p.splits + sp) * MT + g) * kTileM + row) * p.BN + cc);
+                    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+                    for (int sp = 0; sp < p.splits; ++sp) {
+                        const float* src = p.ws + (((size_t)t * p.splits + sp) * MT + g) * kTileM * BN;
 #pragma unroll
-                                for (int j = 0; j < 8; ++j) {
-                                    const float4 x = __ldcg(src + j);
-                                    acc[4 * j] += x.x; acc[4 * j + 1] += x.y; acc[4 * j + 2] += x.z; acc[4 * j + 3] += x.w;
-                                }
+                        for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                const float2 x = __ldcg(reinterpret_cast<const float2*>(src + (size_t)(r0 + 8 * h) * BN + 8 * j + cq));
+                                acc[4 * j + 2 * h] += x.x; acc[4 * j + 2 * h + 1] += x.y;
                             }
-                            uint32_t v0[32];
+                    }
+                }
+            }
+            // ---- one staging box (128 pixels x 128 B = 64 halves / 32 floats of channels) at a time: registers -> + bias ->
+            // activation -> 16-bit -> swizzled shared memory -> TMA store, the store of box b overlapping the math of box b + 1
+            if (reduce_here) {
+                const float* bias_t = bias + n0;
 #pragma unroll
-                            for (int j = 0; j < 32; ++j) v0[j] = __float_as_uint(acc[j]);
-                            epilogue_block<ACT, F32, F16>(v0, bias + n0 + cc, stage_cur + row * 128, (cc - c0) / 8, row, p.act_floor, p.act_slope);
+                for (int bx = 0; bx < nboxes; ++bx, ++box_seq) {
+                    uint8_t* stage_cur = stage_out + g * staging_bytes + (p.out_bufs == 2 ? (box_seq & 1) * box_bytes : 0);
+                    // the store that used this buffer (out_bufs boxes ago) must have finished READING it
+                    if (gtid == 0) {
+                        if (p.out_bufs == 2) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
+                        else asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+                    }
+                    asm volatile("bar.sync %0, 256;" ::"r"(bar_id) : "memory");
+                    if (in_range) stage_box<F32, F16, BN>(acc, bx, bias_t, stage_cur, r0, lane, p.act, p.act_floor, p.act_slope);
+                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic-proxy writes -> visible to the TMA unit
+                    asm volatile("bar.sync %0, 256;" ::"r"(bar_id) : "memory");     // the eight warps of this sub-tile
+                    if (gtid == 0) {
+                        const int cc = n0 + bx * cols_per_box;
+                        if (in_range && cc < p.Cout) {
+                            if (p.flat) tma_store_2d(&map_c, stage_cur, cc, (int)gpix);
+                            else tma_store_4d(&map_c, stage_cur, cc, gwo, gho, img);
                         }
-                    } else if (F32) {
-                        uint32_t v0[32];
-                        B2T_TMEM_LD32(v0, taddr + (uint32_t)c0);
-                        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                        epilogue_block<ACT, F32, F16>(v0, bias + n0 + c0, stage_cur + row * 128, 0, row, p.act_floor, p.act_slope);
-                    } else {
-                        // two 32-column TMEM loads are issued back to back before the wait, so the second overlaps the first's math
-                        uint32_t v0[32], v1[32];
-                        const bool two = c0 + 32 < p.BN;
-                        B2T_TMEM_LD32(v0, taddr + (uint32_t)c0);
-                        if (two) B2T_TMEM_LD32(v1, taddr + (uint32_t)(c0 + 32));
-                        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                        epilogue_block<ACT, F32, F16>(v0, bias + n0 + c0, stage_cur + row * 128, 0, row, p.act_floor, p.act_slope);
-                        if (two) epilogue_block<ACT, F32, F16>(v1, bias + n0 + c0 + 32, stage_cur + row * 128, 4, row, p.act_floor, p.act_slope);
+                        asm volatile("cp.async.bulk.commit_group;" ::: "memory");   // (possibly empty: keeps the wait_group arithmetic uniform)
                     }
-                }
-                if (!SPLIT && bx == nboxes - 1) {
-                    // this warp has read its TMEM lanes: hand the accumulator back to the MMA warp
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    __syncwarp();
-                    if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&tmem_empty[buf])) : "memory");
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic-proxy writes -> visible to the TMA unit
-                asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");     // the four warps of this group
-                if (gtid == 0) {
-                    const int c = n0 + c0;
-                    if (in_range && c < p.Cout) {
-                        if (p.flat) tma_store_2d(&map_c, stage_cur, c, (int)gpix);
-                        else tma_store_4d(&map_c, stage_cur, c, gwo, gho, img);
-                    }
-                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");   // (possibly empty: keeps the wait_group arithmetic uniform)
                 }
             }
         }
         // the staging boxes must outlive the stores' READS of them; the writes themselves are flushed by grid completion like any store
         if (gtid == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == P) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols) : "memory");
     }
 }
 
@@ -769,7 +628,10 @@ CUtensorMapSwizzle swizzle_for(int bk) {
 
 }  // namespace
 
+typedef void (*ConvKernelFn)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const float*, int*, const ConvParams);
+
 struct b2t_conv_plan {
+    ConvKernelFn kernel;           // the instantiation for (fp32 output, fp16, mt, BLOCK_N)
     CUtensorMap map_a, map_b, map_c;
     ConvParams p;
     float* bias_pad;               // plan-owned copy of the bias, zero-padded to whole 32-column epilogue blocks
@@ -784,19 +646,28 @@ struct b2t_conv_plan {
     size_t smem;
 };
 
-typedef void (*ConvKernelFn)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const float*, int*, const ConvParams);
-template <int MT, bool SPLIT>
-ConvKernelFn kernel_for_mt(int act, int f32, int f16) {
-    if (f16) {
-        if (f32) return act ? conv_bias_act_kernel<true, true, true, MT, SPLIT> : conv_bias_act_kernel<false, true, true, MT, SPLIT>;
-        return act ? conv_bias_act_kernel<true, false, true, MT, SPLIT> : conv_bias_act_kernel<false, false, true, MT, SPLIT>;
+template <bool F32, bool F16>
+ConvKernelFn kernel_for_bn(int mt, int bn) {
+    if (mt == 1) {
+        switch (bn) {
+            case 32: return conv_bias_act_kernel<F32, F16, 1, 32>;
+            case 64: return conv_bias_act_kernel<F32, F16, 1, 64>;
+            case 128: return conv_bias_act_kernel<F32, F16, 1, 128>;
+            case 256: return conv_bias_act_kernel<F32, F16, 1, 256>;
+        }
+    } else if (mt == 2) {           // four consumer warpgroups: BLOCK_N <= 128 keeps the accumulators within the register budget
+        switch (bn) {
+            case 32: return conv_bias_act_kernel<F32, F16, 2, 32>;
+            case 64: return conv_bias_act_kernel<F32, F16, 2, 64>;
+            case 128: return conv_bias_act_kernel<F32, F16, 2, 128>;
+        }
     }
-    if (f32) return act ? conv_bias_act_kernel<true, true, false, MT, SPLIT> : conv_bias_act_kernel<false, true, false, MT, SPLIT>;
-    return act ? conv_bias_act_kernel<true, false, false, MT, SPLIT> : conv_bias_act_kernel<false, false, false, MT, SPLIT>;
+    return nullptr;
 }
-ConvKernelFn kernel_for(int act, int f32, int f16, int mt, int split) {
-    if (split) return mt == 2 ? kernel_for_mt<2, true>(act, f32, f16) : kernel_for_mt<1, true>(act, f32, f16);
-    return mt == 2 ? kernel_for_mt<2, false>(act, f32, f16) : kernel_for_mt<1, false>(act, f32, f16);
+// nullptr: no instantiation for this (mt, BLOCK_N)
+ConvKernelFn kernel_for(int f32, int f16, int mt, int bn) {
+    if (f16) return f32 ? kernel_for_bn<true, true>(mt, bn) : kernel_for_bn<false, true>(mt, bn);
+    return f32 ? kernel_for_bn<true, false>(mt, bn) : kernel_for_bn<false, false>(mt, bn);
 }
 
 extern "C" const char* b2t_conv_last_error(void) { return g_conv_err.c_str(); }
@@ -837,7 +708,7 @@ extern "C" int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_
     EncodeTiledFn enc = get_encode();
     if (!enc) return cfail(B2T_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
     b2t_conv_plan* pl = new b2t_conv_plan();
-    pl->bias_pad = nullptr; pl->sched = nullptr; pl->launches = 0; pl->ws = nullptr; pl->flags = nullptr; pl->out = d->y;
+    pl->kernel = nullptr; pl->bias_pad = nullptr; pl->sched = nullptr; pl->launches = 0; pl->ws = nullptr; pl->flags = nullptr; pl->out = d->y;
     ConvParams& p = pl->p;
     p.N = d->n; p.H = d->h; p.W = d->w; p.Cin = d->cin; p.Cout = d->cout;
     p.KH = d->kh; p.KW = d->kw; p.stride = d->stride; p.pad = d->kh / 2; p.pad_w = p.pad;
@@ -854,13 +725,14 @@ extern "C" int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_
     if (bn > 64) bn = (cout_pad % 128 == 0) ? 128 : 64;
     if (d->block_n > 0) bn = d->block_n;
     if (bn % 16 || bn > 256 || bn < 16) { free_plan(pl); return cfail(B2T_EINVAL, "b2t_conv_plan_create: bad BLOCK_N"); }
+    // the kernel is instantiated for BLOCK_N = 32, 64, 128 and 256 (the wgmma N and the accumulator registers are compile-time):
+    // other widths round up, the extra weight rows are zero-filled by the TMA unit and the extra channels clipped on store
+    { int b = 32; while (b < bn) b <<= 1; bn = b; }
     // a store box is 128 bytes of channels (64 halves / 32 floats): N tiles other than the last must be whole boxes,
     // otherwise a tile's last box would spill into its neighbour's channels (the LAST tile is clipped by the map)
     if (bn < cout_pad && bn % (d->out_f32 ? 32 : 64)) { free_plan(pl); return cfail(B2T_EINVAL, "b2t_conv_plan_create: BLOCK_N must be a multiple of 64 (16-bit) / 32 (fp32) when the layer has several N tiles"); }
     p.BN = bn;
-    p.acc_cols = (bn + 31) / 32 * 32;
-    if (2 * MT * p.acc_cols > 512) { free_plan(pl); return cfail(B2T_EINVAL, "b2t_conv_plan_create: 2 x mt x BLOCK_N accumulator columns exceed the 512 TMEM columns"); }
-    { int tc = 32; while (tc < 2 * MT * p.acc_cols) tc <<= 1; p.tmem_cols = tc; }
+    if (MT * bn > 256) { free_plan(pl); return cfail(B2T_EINVAL, "b2t_conv_plan_create: mt x BLOCK_N > 256: the accumulators of four consumer warpgroups exceed the register file"); }
     p.out_pitch = d->out_pitch; p.out_coff = d->out_coff; p.act = d->act == 1 ? 1 : 0; p.act_floor = d->act == 2 ? 0.0f : -INFINITY; p.act_slope = d->act == 3 ? 0.1f : 1.0f; p.out_f32 = d->out_f32; p.f16 = d->io_dtype == B2T_ACT_F16 ? 1 : 0;
     p.flat = (d->kh == 1 && d->stride == 1) ? 1 : 0;
     p.total_pix = (long long)p.N * p.Ho * p.Wo;
@@ -878,8 +750,8 @@ extern "C" int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_
         if (tile_h_px * p.stride > 256) { free_plan(pl); return cfail(B2T_EINVAL, "b2t_conv_plan_create: mt = 2 needs tile_w >= 8 for stride-2 layers (TMA box rows <= 256)"); }
         p.tiles_w = (p.Wo + tile_w_px - 1) / tile_w_px; p.tiles_h = (p.Ho + tile_h_px - 1) / tile_h_px;
     }
-    // flat mode: two K chunks per ring stage when the layer has an even number of 64-channel chunks (bigger TMA boxes: a box is
-    // served at ~460 clk whatever its size up to 32 KB, so 16 KB activation boxes alone cap the fill rate at 45 B/clk)
+    // flat mode: two K chunks per ring stage when the layer has an even number of 64-channel chunks (bigger TMA boxes: a box
+    // costs about the same whatever its size up to tens of KB, so small activation boxes alone cap the fill rate)
     p.kpair = (p.flat && bk == 64 && (p.Cin / bk) % 2 == 0 && d->kpair != 1) ? 2 : 1;
     if (d->kpair == 2 && p.kpair != 2) { free_plan(pl); return cfail(B2T_EINVAL, "b2t_conv_plan_create: kpair = 2 needs a 1x1 / stride 1 layer with an even number of 64-channel chunks"); }
     p.sub_off = halo ? p.TW * bk * 2 : kTileM * bk * 2;
@@ -917,8 +789,8 @@ extern "C" int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_
                 CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     }
     if (r != CUDA_SUCCESS) { free_plan(pl); return cfail(B2T_ECUDA, "cuTensorMapEncodeTiled(A) failed: " + std::to_string((int)r)); }
-    // halo mode: how many filter taps travel in one weight box.  A box is served at ~460 clk whatever its size up to ~32 KB
-    // (profiles/r02_probe_tma_box_size.log), so 16 KB tap tiles (BLOCK_N = 128) fill at 45 B/clk, a kernel row of three (48 KB) at 72.
+    // halo mode: how many filter taps travel in one weight box.  A bulk-tensor copy costs about the same whatever its size up to
+    // tens of KB, so a kernel row of three taps per box fills the ring faster than one tap per box.
     const int kchunks_h = p.Cin / bk;
     const int tiles_n_pre = (cout_pad + bn - 1) / bn;
     int tps = 1;
@@ -987,10 +859,17 @@ extern "C" int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_
     const int box_bytes = kTileM * 128;                  // one staging box: 128 pixels x 64 halves / 32 floats
     p.out_bufs = d->out_bufs == 1 ? 1 : 2;
     auto smem_for = [&](int st) { return (size_t)p.halo_bufs * p.halo_bytes + (size_t)st * stage_bytes + (size_t)MT * p.out_bufs * box_bytes + 512 + 1024; };
-    // Ring depth: what bounds a CTA is the data it keeps in flight (a TMA round trip is ~1-2 k clocks under load, measured:
-    // profiles/r02_probe_*.log), so by default the ring takes the shared memory that is left -- up to kMaxStages -- after
-    // deciding how many CTAs share the SM: 2 when two fit with >= 3 stages each, else 1.
-    const int tmem_ctas = 512 / p.tmem_cols;
+    ConvKernelFn kfn = kernel_for(p.out_f32, p.f16, MT, bn);
+    if (!kfn) { free_plan(pl); return cfail(B2T_EINVAL, "b2t_conv_plan_create: no kernel for this mt / BLOCK_N"); }
+    // the opt-in for > 48 KB of dynamic shared memory is per device and per kernel instantiation
+    if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
+        free_plan(pl); return cfail(B2T_ECUDA, "cannot raise dynamic shared memory for conv kernel");
+    }
+    cudaFuncAttributes fa;
+    if (cudaFuncGetAttributes(&fa, kfn) != cudaSuccess) { free_plan(pl); return cfail(B2T_ECUDA, "cudaFuncGetAttributes(conv kernel) failed"); }
+    // Ring depth: what bounds a CTA is the data it keeps in flight, so by default the ring takes the shared memory that is left --
+    // up to kMaxStages -- after deciding how many CTAs share the SM: 2 when their registers and >= 3 stages each fit, else 1.
+    const bool two_by_regs = 2 * fa.numRegs * (256 * MT + 32 * kMaxProducers) <= 65536;
     int stages = d->stages > 0 ? (d->stages < kMaxStages ? d->stages : kMaxStages) : 0;
     if (p.b_res) stages = 1;
     const int min_stages = (halo || p.kpair == 2) ? 2 : 3;
@@ -998,7 +877,7 @@ extern "C" int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_
         for (int pass = 0; pass < 2 && stages == 0; ++pass) {
             int per2 = 0, per1 = 0;
             for (int st = kMaxStages; st >= 1; --st) { if (!per2 && smem_for(st) <= 113 * 1024) per2 = st; if (!per1 && smem_for(st) <= 226 * 1024) per1 = st; }
-            const int pick = (tmem_ctas >= 2 && MT == 1 && per2 >= 3) ? per2 : per1;
+            const int pick = (two_by_regs && MT == 1 && per2 >= 3) ? per2 : per1;
             if (pick >= min_stages || p.out_bufs == 1 || d->out_bufs == 2) stages = pick;
             else p.out_bufs = 1;                          // a second staging box is worth less than a ring stage
         }
@@ -1008,40 +887,27 @@ extern "C" int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_
     if (smem_for(stages) > 226 * 1024 && p.out_bufs == 2) p.out_bufs = 1;
     if (smem_for(stages) > 227 * 1024) { free_plan(pl); return cfail(B2T_EINVAL, "b2t_conv_plan_create: tile does not fit in shared memory (reduce BLOCK_N, mt or tps)"); }
     if (halo && d->halo_bufs == 3 && smem_for(stages) + p.halo_bytes <= 226 * 1024) p.halo_bufs = 3;
-    int ctas_per_sm = (int)((227 * 1024) / smem_for(stages));
-    if (ctas_per_sm > tmem_ctas) ctas_per_sm = tmem_ctas;
-    if (ctas_per_sm > (MT == 1 ? 2 : 1)) ctas_per_sm = MT == 1 ? 2 : 1;        // register budget of the kernel's launch bounds
     // a producer that skips the other producer's steps only checks the PARITY of its stage's barrier: with fewer stages than
     // producers it could run two phases ahead of a stage and alias it -- never more producers than stages
     const int P_eff = P > stages ? stages : P;
     p.P = P_eff;
-    const int threads = 32 * (P_eff + 1) + 128 * MT;
-    if (ctas_per_sm * threads > 2048 - 64) ctas_per_sm = (2048 - 64) / threads;
-    if (ctas_per_sm < 1) ctas_per_sm = 1;
+    const int threads = 256 * MT + 32 * P_eff;
     p.stages = stages;
     pl->smem = smem_for(stages);
     pl->threads = threads;
+    int ctas_per_sm = 1;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, kfn, threads, pl->smem) != cudaSuccess || ctas_per_sm < 1) ctas_per_sm = 1;
     p.tiles_m = p.flat ? (int)((p.total_pix + kTileM * MT - 1) / (kTileM * MT)) : p.N * p.tiles_w * p.tiles_h;
     p.tiles_n = (cout_pad + bn - 1) / bn;
-    int n_sm = 148;
+    int n_sm = 132;
     { int devid = 0; cudaGetDevice(&devid); int v = 0; if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, devid) == cudaSuccess && v > 0) n_sm = v; }
     const long long total_units = (long long)p.tiles_m * p.tiles_n * splits;
     if (total_units > 0x7fffffff) { free_plan(pl); return cfail(B2T_EINVAL, "b2t_conv_plan_create: too many tiles"); }
     long long g = (long long)n_sm * ctas_per_sm;
     if (g > total_units) g = total_units;
     pl->grid = dim3((unsigned)g, 1, 1);
-    {   // the opt-in for > 48 KB of dynamic shared memory is per device and per kernel instantiation
-        static bool attr_set[64] = {};
-        int devid = 0; cudaGetDevice(&devid);
-        if (devid < 0 || devid >= 64 || !attr_set[devid]) {
-            for (int v = 0; v < 32; ++v)
-                if (cudaFuncSetAttribute(kernel_for(v & 1, (v >> 1) & 1, (v >> 2) & 1, 1 + ((v >> 3) & 1), v >> 4), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
-                    free_plan(pl); return cfail(B2T_ECUDA, "cannot raise dynamic shared memory for conv kernel");
-                }
-            if (devid >= 0 && devid < 64) attr_set[devid] = true;
-        }
-    }
-    {   // the epilogue reads the bias as float4 without bounds checks: snapshot it into a zero-padded array
+    pl->kernel = kfn;
+    {   // the epilogue reads the bias in pairs without bounds checks: snapshot it into a zero-padded array
         const size_t nb = (size_t)p.tiles_n * bn + 64;
         if (cudaMalloc(&pl->bias_pad, nb * sizeof(float)) != cudaSuccess) { free_plan(pl); return cfail(B2T_ECUDA, "cudaMalloc(bias) failed"); }
         if (cudaMemset(pl->bias_pad, 0, nb * sizeof(float)) != cudaSuccess ||
@@ -1059,10 +925,7 @@ extern "C" int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_
             free_plan(pl); return cfail(B2T_ECUDA, "cudaMalloc(split-K workspace) failed");
         }
     }
-    p.ws = pl->ws; p.flags = pl->flags; p.trace = nullptr;
-#ifdef B2T_CONV_TRACE
-    if (cudaMalloc(&p.trace, (size_t)g * 16 * sizeof(long long)) == cudaSuccess) cudaMemset(p.trace, 0, (size_t)g * 16 * sizeof(long long));
-#endif
+    p.ws = pl->ws; p.flags = pl->flags;
     *out_plan = pl;
     return B2T_OK;
 }
@@ -1074,20 +937,10 @@ extern "C" double b2t_conv_plan_flops(const b2t_conv_plan* pl) { return pl ? pl-
 extern "C" int b2t_conv_plan_info(const b2t_conv_plan* pl, int* out, int n) {
     if (!pl || !out) return cfail(B2T_EINVAL, "b2t_conv_plan_info: null argument");
     const ConvParams& p = pl->p;
-    const int v[17] = {(int)pl->grid.x, pl->threads, (int)pl->smem, p.BN, p.stages, p.MT, p.splits, p.halo, p.halo_bufs, p.tiles_m, p.tiles_n, p.tmem_cols, p.P,
+    const int v[17] = {(int)pl->grid.x, pl->threads, (int)pl->smem, p.BN, p.stages, p.MT, p.splits, p.halo, p.halo_bufs, p.tiles_m, p.tiles_n, p.BN / 2, p.P,
                        p.tps, p.b_res, p.out_bufs, p.kpair};
     for (int i = 0; i < n && i < 17; ++i) out[i] = v[i];
     return B2T_OK;
-}
-
-extern "C" int b2t_conv_plan_trace(const b2t_conv_plan* pl, long long* out_host, int max_ctas) {
-    // B2T_CONV_TRACE builds only: copies (and clears) the per-CTA cycle counters; returns the number of CTAs, 0 when tracing is off
-    if (!pl || !pl->p.trace) return 0;
-    int n = (int)pl->grid.x < max_ctas ? (int)pl->grid.x : max_ctas;
-    cudaDeviceSynchronize();
-    cudaMemcpy(out_host, pl->p.trace, (size_t)n * 16 * sizeof(long long), cudaMemcpyDeviceToHost);
-    cudaMemset(pl->p.trace, 0, (size_t)pl->grid.x * 16 * sizeof(long long));
-    return n;
 }
 
 extern "C" int b2t_conv_run(const b2t_conv_plan* pl, void* stream) {
@@ -1099,7 +952,7 @@ extern "C" int b2t_conv_run(const b2t_conv_plan* pl, void* stream) {
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = use_pdl ? 1 : 0;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kernel_for(pl->p.act, pl->p.out_f32, pl->p.f16, pl->p.MT, pl->p.splits > 1), pl->map_a, pl->map_b, pl->map_c, (const float*)pl->bias_pad,
+    cudaError_t e = cudaLaunchKernelEx(&cfg, pl->kernel, pl->map_a, pl->map_b, pl->map_c, (const float*)pl->bias_pad,
                                        pl->sched + 2 * (pl->launches++ & 3u), pl->p);
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e != cudaSuccess) return cfail(B2T_ECUDA, std::string("conv launch: ") + cudaGetErrorString(e));

@@ -191,7 +191,7 @@ __global__ void detect_decode_kernel(const float* __restrict__ raw, int rp, floa
     }
 }
 
-inline int grid_for(long long total, int block) { long long g = (total + block - 1) / block; return (int)(g > 148 * 32 ? 148 * 32 : (g < 1 ? 1 : g)); }
+inline int grid_for(long long total, int block) { long long g = (total + block - 1) / block; return (int)(g > 132 * 32 ? 132 * 32 : (g < 1 ? 1 : g)); }
 }  // namespace
 
 extern "C" const char* b2t_detect_last_error(void) { return g_det_err.c_str(); }

@@ -157,8 +157,8 @@ __global__ void fast_score_kernel(unsigned char* ws, GmcGeom g) {
             for (int k = 0; k < 16; ++k) { nb += d[k] > kFastThreshold; nd += -d[k] > kFastThreshold; }
             if (nb >= 9 || nd >= 9) {
                 // min over the arc k .. k+8 (cyclic) by doubling -- m2, m4, m8, then the ninth element -- once on d = v - p and
-                // once on e = p - v.  (Deliberately NOT "-max(d)" for the dark arcs: nvcc 12.9 / sm_100a fuses max(best, mn, -mx)
-                // into VIMNMX3 and drops the negation -- measured on a B200, tools/gmc_debug.py.)
+                // once on e = p - v.  (Deliberately NOT "-max(d)" for the dark arcs: nvcc 12.9 has been seen to fuse max(best, mn, -mx)
+                // into a three-way VIMNMX3 and drop the negation, tools/gmc_debug.py.)
                 int e[16];
 #pragma unroll
                 for (int k = 0; k < 16; ++k) e[k] = -d[k];
@@ -684,7 +684,7 @@ extern "C" int b2t_gmc_reset(void* workspace, int n_seq, int height, int width, 
 namespace {
 int prepare(const unsigned char* frames_bgr, const GmcGeom& g, unsigned char* ws, cudaStream_t s) {
     const int px = g.h * g.w;
-    const int gx = (px + 255) / 256 < 148 * 8 ? (px + 255) / 256 : 148 * 8;
+    const int gx = (px + 255) / 256 < 132 * 8 ? (px + 255) / 256 : 132 * 8;
     // cv::resize derives the scales from inv_scale = dsize / ssize in double: scale = 1. / inv_scale
     const double scale_x = 1.0 / ((double)g.w / (double)g.src_w), scale_y = 1.0 / ((double)g.h / (double)g.src_h);
     B2T_LAUNCH(gray_kernel, dim3(gx, g.n_seq), 256, 0, s, frames_bgr, ws, g, scale_x, scale_y);
@@ -697,7 +697,7 @@ int estimate(const GmcGeom& g, unsigned char* ws, const float* dets, const int* 
     B2T_LAUNCH(nms_flag_kernel, dim3(g.h, g.n_seq), 128, 0, s, ws, g, dets, det_counts, dmax, det_thresh);
     B2T_LAUNCH(scan_rows_kernel, dim3(1, g.n_seq), 1024, 0, s, ws, g);
     B2T_LAUNCH(compact_kernel, dim3((g.h + 3) / 4, g.n_seq), 128, 0, s, ws, g);
-    const int kpb = (g.max_kp + 7) / 8 < 148 * 4 ? (g.max_kp + 7) / 8 : 148 * 4;
+    const int kpb = (g.max_kp + 7) / 8 < 132 * 4 ? (g.max_kp + 7) / 8 : 132 * 4;
     B2T_LAUNCH(describe_kernel, dim3(kpb, g.n_seq), 256, 0, s, ws, g);
     B2T_LAUNCH(match_kernel, dim3((g.max_kp + 127) / 128, g.n_seq, kSplit), 128, 0, s, ws, g);
     B2T_LAUNCH(filter_kernel, dim3(g.n_seq), kEstThreads, 0, s, ws, g);

@@ -375,7 +375,7 @@ extern "C" int b2t_detect_nms(const b2t_head_level* levels, int n_levels, int B,
     cudaMemsetAsync(ws.count, 0, ws.zero_bytes, s);
     const long long total = (long long)B * L.per_image;
     long long g = (total + 255) / 256;
-    if (g > 148 * 16) g = 148 * 16;
+    if (g > 132 * 16) g = 132 * 16;
     B2T_LAUNCH(filter_raw_kernel, (int)g, 256, 0, s, L, B, no, conf_thres, bn, ws.cand, ws.count, ws.hist, max_cand);
     return sort_and_select(ws, B, iou_thres, max_det, max_nms, max_cand, post, gain, padw, padh, img_w, img_h, out, out_count, s);
 }

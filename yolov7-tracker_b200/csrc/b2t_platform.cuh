@@ -1,6 +1,6 @@
 // b2t_platform.cuh -- compile-target glue for the tracker kernels.
 //
-// Product build: nvcc, sm_100a (see build.py).  The B2T_HOSTSIM branch is used ONLY by
+// Product build: nvcc, sm_90a (see build.py).  The B2T_HOSTSIM branch is used ONLY by
 // tests/hostsim (a fiber-based single-block simulator for the GPU-less CI tier); the shipped
 // library is never built with it.
 #pragma once
@@ -23,8 +23,7 @@
 #endif
 
 #define B2T_DEV __device__ __forceinline__
-// Out-of-line device functions were tried for the big phases (the fused kernel is ~300-570 KB of
-// SASS) and measured 1.6x SLOWER on B200: the by-reference work structs move to local memory under
-// the ABI.  Everything is force-inlined; stall_no_inst is < 8 % of samples (profiles/).
+// Everything is force-inlined: out-of-line device functions for the big phases would move their
+// by-reference work structs to local memory under the ABI.
 #define B2T_DEVNI __device__ __forceinline__
 #define B2T_FULL 0xffffffffu

@@ -173,7 +173,7 @@ int launch_check(const char* what) {
     if (e != cudaSuccess) { b2t::set_detect_error((std::string(what) + ": " + cudaGetErrorString(e)).c_str()); return B2T_ECUDA; }
     return B2T_OK;
 }
-int grid_of(long long total) { long long g = (total + 255) / 256; return (int)(g > 148 * 16 ? 148 * 16 : (g < 1 ? 1 : g)); }
+int grid_of(long long total) { long long g = (total + 255) / 256; return (int)(g > 132 * 16 ? 132 * 16 : (g < 1 ? 1 : g)); }
 }  // namespace
 
 extern "C" int b2t_letterbox(const unsigned char* bgr, int B, int src_h, int src_w, int src_pitch, int unpad_w, int unpad_h, int top, int left,

@@ -1,6 +1,6 @@
 // b2t_reid.cu -- glue kernels of the appearance branch (SURVEY.md section 8f row 3): everything of the reference's ReID extractor
 // (tracker/reid_models/deepsort_reid.py:63-153) that is not a convolution.  The 3x3 / 1x1 convolutions (+ folded BatchNorm + ReLU) run on
-// the tcgen05 kernel of b2t_conv.cu; these kernels are the byte / element-wise work around them -- HBM-bound, 16-byte vectors.
+// the wgmma kernel of b2t_conv.cu; these kernels are the byte / element-wise work around them -- HBM-bound, 16-byte vectors.
 //   reid_crop_kernel       Extractor._preprocess :134-146: crop.astype(float32) / 255 -> cv2.resize to 64 x 128 (bilinear, float) ->
 //                          ToTensor -> Normalize(mean, std); written as NHWC 16-bit with the 3 channels padded to 16 (tensor-core K granularity)
 //   maxpool3x3s2_kernel    nn.MaxPool2d(3, 2, padding=1) :72
@@ -23,7 +23,7 @@ int rcheck(const char* what) {
     if (e != cudaSuccess) { b2t::set_detect_error((std::string(what) + ": " + cudaGetErrorString(e)).c_str()); return B2T_ECUDA; }
     return B2T_OK;
 }
-int grid_for(long long total, int block) { long long g = (total + block - 1) / block; return (int)(g > 148 * 16 ? 148 * 16 : (g < 1 ? 1 : g)); }
+int grid_for(long long total, int block) { long long g = (total + block - 1) / block; return (int)(g > 132 * 16 ? 132 * 16 : (g < 1 ? 1 : g)); }
 
 __device__ __forceinline__ float load16(const unsigned short* p, int f16) {
     return f16 ? __half2float(*reinterpret_cast<const __half*>(p)) : __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(p));
@@ -199,7 +199,7 @@ extern "C" int b2t_batchnorm_batch_stats(const void* x, void* y, long long n_pix
     if (threads % cv) return rfail(B2T_EINVAL, "b2t_batchnorm_batch_stats: c / 8 must divide 256");
     const long long ppb = threads / cv;
     long long g = (n_pix + ppb * 16 - 1) / (ppb * 16);
-    g = g < 1 ? 1 : (g > 148 * 8 ? 148 * 8 : g);
+    g = g < 1 ? 1 : (g > 132 * 8 ? 132 * 8 : g);
     bn_stats_kernel<<<(int)g, threads, 0, s>>>((const unsigned short*)x, n_pix, c, sums_ws, act_dtype == B2T_ACT_F16);
     bn_apply_kernel<<<grid_for(n_pix * cv, 256), 256, 0, s>>>((const unsigned short*)x, (unsigned short*)y, n_pix * cv, c, n_pix, sums_ws, gamma, beta, eps, relu,
                                                            act_dtype == B2T_ACT_F16);

@@ -434,13 +434,22 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         sm.detbox[4 * i + 2] = (T)(w + d[0]);                   // .tlbr: tlwh[2:] += tlwh[:2], float32
         sm.detbox[4 * i + 3] = (T)(h + d[1]);
     }
+    // Deliberate divergence from the reference, limited to the boxes it cannot track: a detection with a non-finite coordinate, zero
+    // height (xyah: no aspect ratio, and the Kalman noise scaled by the height vanishes -> NaN state / a failed Cholesky factorisation)
+    // or, with the xywh filter, zero width, takes no part.  Every other box -- zero width under xyah included -- is tracked as the
+    // reference tracks it.
+    auto has_area = [&](int i) {
+        const float* d = dets + 6 * i;
+        for (int j = 0; j < 4; ++j) if (!(d[j] - d[j] == 0.f)) return false;    // NaN or infinite coordinate (x - x is NaN)
+        return d[3] - d[1] != 0.f && (p.fmt != FMT_XYWH || d[2] - d[0] != 0.f);
+    };
     int nhi, nlo;
     if (p.kind == KIND_SORT) {
-        nhi = block_compact(nd, [&](int i) { return dets[6 * i + 4] > p.det_thresh; }, sm.hi, sm.misc);
+        nhi = block_compact(nd, [&](int i) { return dets[6 * i + 4] > p.det_thresh && has_area(i); }, sm.hi, sm.misc);
         nlo = 0;
     } else {
-        nhi = block_compact(nd, [&](int i) { return dets[6 * i + 4] >= p.det_thresh; }, sm.hi, sm.misc);
-        nlo = block_compact(nd, [&](int i) { const float s = dets[6 * i + 4]; return !(s >= p.det_thresh) && s > p.low_thresh; },
+        nhi = block_compact(nd, [&](int i) { return dets[6 * i + 4] >= p.det_thresh && has_area(i); }, sm.hi, sm.misc);
+        nlo = block_compact(nd, [&](int i) { const float s = dets[6 * i + 4]; return !(s >= p.det_thresh) && s > p.low_thresh && has_area(i); },
                             sm.lo, sm.misc);
     }
 

@@ -1,6 +1,6 @@
 // b2t_tracker.cu -- kernels + C ABI (include/b200track.h) for the association branch:
 // batched Kalman ops, "+1" IoU cost, thresholded exact assignment and the fused per-frame
-// SORT / ByteTrack / BoT-SORT step.  Compiled for sm_100a with --fmad=false (see b2t_iou.cuh).
+// SORT / ByteTrack / BoT-SORT step.  Compiled for sm_90a with --fmad=false (see b2t_iou.cuh).
 #include <string>
 #include <cstdio>
 #include <cstdlib>

@@ -1,4 +1,4 @@
-"""``attempt_load`` (reference models/experimental.py:83-106) for the B200 detector.
+"""``attempt_load`` (reference models/experimental.py:83-106) for the H100 detector.
 
 The reference un-pickles a whole ``nn.Module`` from the checkpoint (key 'ema' or 'model').  Pickled reference modules
 cannot be loaded without the reference's own class definitions, so this loader accepts

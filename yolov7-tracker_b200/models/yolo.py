@@ -6,7 +6,7 @@ eval-mode ``models.yolo.Model`` the tracker driver uses (tracker/track.py:82-84,
     out = model(img.to(device))[0]                          # (B, N, 5 + nc) float32
 
 Two deploy graphs are built: YOLOv7-w6 (cfg/deploy/yolov7-w6.yaml, what the tracker driver loads) and YOLOv7-tiny
-(cfg/deploy/yolov7-tiny.yaml, BASELINE.json configs[0]); the forward runs on the tcgen05 conv kernels through
+(cfg/deploy/yolov7-tiny.yaml, BASELINE.json configs[0]); the forward runs on the wgmma conv kernels through
 ``b200track.detector.DetectorW6`` / ``b200track.tiny.DetectorTiny``.  Engines are built lazily per (batch, image size)."""
 import torch
 
@@ -21,7 +21,7 @@ class Model(torch.nn.Module):
         super().__init__()
         self.tiny = "tiny" in str(cfg)
         if "w6" not in str(cfg) and not self.tiny:
-            raise NotImplementedError("only the YOLOv7-w6 and YOLOv7-tiny deploy graphs are built for B200 (SURVEY.md 8a a1)")
+            raise NotImplementedError("only the YOLOv7-w6 and YOLOv7-tiny deploy graphs are built for the GPU (SURVEY.md 8a a1)")
         if nc not in (None, NC):
             raise NotImplementedError("nc = %d heads only" % NC)
         self.yaml = {"nc": NC, "anchors": _tiny.ANCHORS if self.tiny else ANCHORS}

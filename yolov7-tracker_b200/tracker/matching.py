@@ -77,7 +77,7 @@ _cos_gemm = None
 
 
 def cal_cosine_distance(mat1, mat2):
-    """normalize(mat1) @ normalize(mat2).T (reference :165-178) on the tcgen05 conv kernel as a split-fp16 GEMM
+    """normalize(mat1) @ normalize(mat2).T (reference :165-178) on the wgmma conv kernel as a split-fp16 GEMM
     (b200track/gemm.py): float64-level results (~1e-6) from the tensor cores."""
     global _cos_gemm
     ops = _eng.ops()

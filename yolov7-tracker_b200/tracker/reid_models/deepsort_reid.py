@@ -2,7 +2,7 @@
 ``__call__(im_crops) -> (n, 512) float32 ndarray`` (reference :109-153), imported by ``basetrack`` / ``botsort`` / ``deepsort`` /
 ``strongsort`` as ``from reid_models.deepsort_reid import Extractor``.
 
-The network (``Net(reid=True)``, :63-106) runs on the GPU through ``b200track/reid.py``: convolutions on the tcgen05 kernel, the
+The network (``Net(reid=True)``, :63-106) runs on the GPU through ``b200track/reid.py``: convolutions on the wgmma kernel, the
 rest as element-wise kernels (csrc/b2t_reid.cu).  The reference never switches its network to ``eval()``, so its BatchNorm layers use
 the statistics of the crops of each call; ``bn_mode='batch'`` (default) reproduces that, ``'running'`` is eval-mode BatchNorm."""
 import os

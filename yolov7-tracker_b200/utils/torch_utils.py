@@ -6,7 +6,7 @@ import torch
 
 def select_device(device='', batch_size=None):
     if str(device).lower() == 'cpu' or not torch.cuda.is_available():
-        raise RuntimeError("the B200 detector path has no CPU fallback: a CUDA device is required")
+        raise RuntimeError("the GPU detector path has no CPU fallback: a CUDA device is required")
     idx = 0 if device in ('', None) else int(str(device).split(',')[0])
     return torch.device('cuda:%d' % idx)
 
@@ -18,7 +18,7 @@ def time_synchronized():
 
 
 class TracedModel(torch.nn.Module):
-    """The reference wraps the model in a torch.jit trace (utils/torch_utils.py:343-373); the B200 forward is a fixed
+    """The reference wraps the model in a torch.jit trace (utils/torch_utils.py:343-373); the GPU forward is a fixed
     launch sequence already, so the wrapper only forwards."""
 
     def __init__(self, model=None, device=None, img_size=(640, 640)):
