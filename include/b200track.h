@@ -186,9 +186,11 @@ const char* b2t_conv_last_error(void);
 int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_plan);
 void b2t_conv_plan_destroy(b2t_conv_plan* plan);
 double b2t_conv_plan_flops(const b2t_conv_plan* plan);
-/* launch geometry chosen at plan time: out[0..17) = grid, threads, dynamic smem bytes, BLOCK_N, ring stages, mt, splits, halo,
+/* launch geometry chosen at plan time: out[0..18) = grid, threads, dynamic smem bytes, BLOCK_N, ring stages, mt, splits, halo,
  * halo buffers, tiles_m, tiles_n, accumulator registers per consumer thread, producer warps, taps per stage, resident weights, staging boxes,
- * K chunks per stage (diagnostics for the autotuner and the per-layer tables). */
+ * K chunks per stage, consumer schedule (1 = ping-pong: each consumer warpgroup owns whole 128-pixel tiles and the two alternate, so one
+ * warpgroup's epilogue overlaps the other's MMAs -- MT = 1 with BLOCK_N <= 128; 0 = cooperative: two warpgroups per 128-pixel sub-tile)
+ * (diagnostics for the autotuner and the per-layer tables). */
 int b2t_conv_plan_info(const b2t_conv_plan* plan, int* out, int n);
 int b2t_conv_run(const b2t_conv_plan* plan, void* stream);
 

@@ -1,7 +1,9 @@
 """GPU box: per-conv-launch table of one detector step (batch 8, 1280 x 1280) WITHOUT a profiler: the autotuned configuration of
 every launch, its time alone (back-to-back CUDA-event timing, the autotuner's own number) and its time INSIDE the step
 (difference between the CUDA graphs of ops[0..k] and ops[0..k-1], programmatic dependent launch overlap included), next to the
-layer's floors: flops / sustained tensor peak and algorithmic bytes / HBM peak (MEASURED_PEAKS.json).
+layer's floors: flops / sustained tensor peak and algorithmic bytes / HBM peak (MEASURED_PEAKS.json, else the H100 SXM data sheet:
+989 TFLOP/s dense fp16, 3 350 GB/s -- a power-capped card reaches less, so the floors are optimistic there).  'pp' / 'co' = consumer
+schedule: ping-pong (one warpgroup's epilogue under the other's MMAs) or cooperative.
 
     python tools/conv_graph_table.py [out.txt]
 """
@@ -43,7 +45,7 @@ def main(out_path=None, batch=8, size=1280):
     sd = calibrated_state_dict(0, size, dev)
     det = DetectorW6(sd, batch=batch, img_size=size, device=dev, use_graph=False)
     peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-    peak, hbm = float(peaks.get("bf16_tflops_sustained", 1361.1)) * 1e12, float(peaks.get("hbm_gbs", 6577.4)) * 1e9
+    peak, hbm = float(peaks.get("bf16_tflops_sustained", 989.0)) * 1e12, float(peaks.get("hbm_gbs", 3350.0)) * 1e9
     fns = [fn for fn, _, _ in det.ops]
     plans = [p for p in det.keep if hasattr(p, "geom")]
     out, tot_in, tot_alone, tot_floor, worst, pi = [], 0.0, 0.0, 0.0, (0.0, ""), 0
@@ -62,15 +64,16 @@ def main(out_path=None, batch=8, size=1280):
         by = g["n"] * (g["h"] * g["w"] * cin * 2 + ho * wo * g["cout"] * (4 if g["out_f32"] else 2)) + g["k"] * g["k"] * cin * g["cout"] * 2
         tf, th = fl / peak * 1e6, by / hbm * 1e6
         floor, alone = max(tf, th), t.get("us", float("nan"))
-        cfg = "%4d>%4d k%d s%d %3dx%-3d bn%3d mt%d st%d v%d g%3d" % (g["cin"], g["cout"], g["k"], g["stride"], g["h"], g["w"], inf["bn"], inf["mt"], inf["stages"], t.get("variant", 0), inf["grid"])
-        out.append("%-24s %-48s alone %6.1f  in-graph %6.1f us %6.0f TFLOP/s  floor %6.1f (%s) x%4.1f" %
+        cfg = "%4d>%4d k%d s%d %3dx%-3d bn%3d mt%d %s st%d v%d g%3d" % (g["cin"], g["cout"], g["k"], g["stride"], g["h"], g["w"], inf["bn"], inf["mt"],
+                                                             "pp" if inf["pingpong"] else "co", inf["stages"], t.get("variant", 0), inf["grid"])
+        out.append("%-24s %-51s alone %6.1f  in-graph %6.1f us %6.0f TFLOP/s  floor %6.1f (%s) x%4.1f" %
                    (name.replace("model.", "L").replace(".conv", ""), cfg, alone, d_us, fl / max(d_us, 1e-3) / 1e6, floor, "tensor" if tf >= th else "hbm", d_us / floor))
         tot_in += d_us; tot_alone += alone; tot_floor += floor
         if d_us / floor > worst[0]:
             worst = (d_us / floor, name)
     hdr = ["# one detector step, batch %d, %dx%d, fp16 activations: autotuned configuration per conv launch; 'alone' = back-to-back launches of that" % (batch, size, size),
            "# plan (CUDA events), 'in-graph' = graph(ops[0..k]) - graph(ops[0..k-1]) (what the launch adds to the step, PDL overlap included);",
-           "# floor = max(flops / %.0f TFLOP/s sustained, algorithmic bytes / %.0f GB/s), MEASURED_PEAKS.json" % (peak / 1e12, hbm / 1e9)]
+           "# floor = max(flops / %.0f TFLOP/s, algorithmic bytes / %.0f GB/s) (MEASURED_PEAKS.json, else the H100 SXM data sheet)" % (peak / 1e12, hbm / 1e9)]
     tail = ["# conv launches: in-graph %.1f us, alone %.1f us, sum of floors %.1f us; worst launch x%.1f (%s); whole forward graph %.1f us" %
             (tot_in, tot_alone, tot_floor, worst[0], worst[1], prev * 1e3)]
     text = "\n".join(hdr + out + tail)

@@ -52,9 +52,9 @@ class ConvPlan:
         if rc != 0:
             raise L.B2TError("b2t_conv_plan_create: %s" % (self.lib.b2t_conv_last_error() or b"").decode())
         self.flops = self.lib.b2t_conv_plan_flops(self.handle)
-        info = (C.c_int * 17)()
-        self.lib.b2t_conv_plan_info(self.handle, info, 17)
-        self.info = dict(zip(("grid", "threads", "smem", "bn", "stages", "mt", "splits", "halo", "halo_bufs", "tiles_m", "tiles_n", "acc_regs", "producers", "tps", "b_res", "out_bufs", "kpair"), list(info)))
+        info = (C.c_int * 18)()
+        self.lib.b2t_conv_plan_info(self.handle, info, 18)
+        self.info = dict(zip(("grid", "threads", "smem", "bn", "stages", "mt", "splits", "halo", "halo_bufs", "tiles_m", "tiles_n", "acc_regs", "producers", "tps", "b_res", "out_bufs", "kpair", "pingpong"), list(info)))
 
     def run(self, stream=None):
         s = C.c_void_p(torch.cuda.current_stream().cuda_stream if stream is None else stream)

@@ -249,8 +249,8 @@ class DetectorW6:
 
     def _tuned_plan(self, src, variants, b, dst, hw_in, cin, cout, k, s, act, f32):
         """Plan-time autotuning: the kernel's best tiling depends on the layer -- tile width BLOCK_N, one or two 128-pixel
-        sub-tiles per tile (mt), ring depth (0 = as deep as shared memory allows, 2 / 3 = shallow rings that let two CTAs share an
-        SM) and the addressing variant -- so each candidate is timed with CUDA events on the real buffers and the fastest kept
+        sub-tiles per tile (mt), ring depth (0 = as deep as shared memory allows, 2 / 3 = shallow rings) and the addressing
+        variant -- so each candidate is timed with CUDA events on the real buffers and the fastest kept
         (tools/conv_layer_bench.py prints the whole table).  ``variants``: [(packed weights, extra ConvPlan arguments)]."""
         cout_pad = (cout + 15) // 16 * 16
         shapes = [dict()]

@@ -17,12 +17,16 @@
 //     map's element strides, and the box lands in shared memory as 128 rows of BK*2 bytes with the
 //     128-/64-/32-byte swizzle -- exactly the canonical K-major wgmma operand layout.  No im2col.
 //   * B operand: 2-D map (K, Cout), box {BK, BLOCK_N}.
-//   * warps [0, 8 MT) are the consumers: two warpgroups per 128-pixel sub-tile, each issuing
-//     wgmma.mma_async m64 x BLOCK_N x k16 on its 64 pixel rows with the accumulator in registers, then the epilogue
-//     from those registers: +bias -> SiLU (one tanh.approx on the SFU) -> fp16 / bf16 (or fp32) -> 128-byte-swizzled
+//   * warps [0, 8 MT) are the consumers, issuing wgmma.mma_async m64 x BLOCK_N x k16 with the accumulators in registers, then
+//     the epilogue from those registers: +bias -> SiLU (one tanh.approx on the SFU) -> fp16 / bf16 (or fp32) -> 128-byte-swizzled
 //     staging tile -> TMA bulk tensor STORES straight into the consumer's concat buffer
-//     (concat-by-address; partial tiles and the 255-channel head are clipped by the TMA unit).
-//     The warps after them are TMA producers.
+//     (concat-by-address; partial tiles and the 255-channel head are clipped by the TMA unit).  Two schedules, fixed by (MT, BLOCK_N):
+//       - PING-PONG (MT = 1, BLOCK_N <= 128): each of the two warpgroups owns WHOLE 128-pixel tiles (both m64 halves) and they take
+//         alternate tiles; a turn barrier pair orders their MMA loops, so one warpgroup's epilogue runs under the other's MMAs.
+//       - COOPERATIVE (MT = 2, or BLOCK_N = 256): two warpgroups per 128-pixel sub-tile, one m64 half each, epilogue together.
+//     Both sum every output in the same K order, so the schedule changes the time, never a result bit.
+//   * the warpgroup after the consumers is the producer warpgroup: 1 or 2 of its warps issue TMA copies, and it hands most of
+//     its registers to the consumers (setmaxnreg), which is what lets a warpgroup hold 128 x 128 or 64 x 256 accumulators unspilled.
 //   * PERSISTENT: the grid is (#SMs x CTAs/SM); a CTA draws every tile, the first one included, from a global
 //     ticket counter (N tile fastest, so neighbouring CTAs share the A tile in L2); the first producer warp publishes every tile
 //     index to the other warps through a small mbarrier-guarded ring in shared memory.  The operand ring (full/empty mbarriers)
@@ -49,7 +53,18 @@ constexpr int kMaxStages = 8;
 constexpr int kTileM = 128;        // pixels per sub-tile = rows of two m64 wgmma warpgroups
 constexpr int kMaxHalo = 3;        // halo-tile buffers (halo mode)
 constexpr int kRing = 4;           // tile-index ring depth (the producer runs at most a few tiles ahead)
-constexpr int kMaxProducers = 2;   // warps [8 MT, 8 MT + P) = TMA producers after the 8 consumer warps per sub-tile
+constexpr int kMaxProducers = 2;   // warps [8 MT, 8 MT + P) of the producer warpgroup issue TMA copies; the others idle
+
+// the consumer schedule is a function of the instantiation (see the header); the host sizes the staging boxes from it
+__host__ __device__ constexpr bool ping_pong(int mt, int bn) { return mt == 1 && bn <= 128; }
+// register budget: one CTA per SM.  ptxas sizes the launch allocation from __launch_bounds__ (65536 / threads, rounded down to 8
+// per thread); the producer warpgroup lowers its limit with setmaxnreg.dec and the consumers raise theirs by what that freed inside
+// the CTA: 168 -> 224 with 384 threads (MT = 1), 96 -> 104 with 640 (MT = 2).  48 is the least the producer code runs in unspilled.
+__host__ __device__ constexpr int conv_threads(int mt) { return 256 * mt + 128; }
+__host__ __device__ constexpr int launch_regs(int mt) { return 65536 / conv_threads(mt) / 8 * 8; }
+constexpr int kProducerRegs = 48;
+__host__ __device__ constexpr int consumer_regs(int mt) { return (launch_regs(mt) + (launch_regs(mt) - kProducerRegs) * 128 / (256 * mt)) / 8 * 8; }
+static_assert(consumer_regs(1) == 224 && consumer_regs(2) == 104, "register hand-off");
 
 struct ConvParams {
     int N, H, W, Cin;              // input geometry (Cin = channels of the slice read)
@@ -141,10 +156,15 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // keeps the compiler from moving accumulator accesses across wgmma fences / waits
-template <int R> __device__ __forceinline__ void acc_fence(float (&d)[R]) {
+template <int H, int R> __device__ __forceinline__ void acc_fence(float (&d)[H][R]) {
 #pragma unroll
-    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+    for (int h = 0; h < H; ++h)
+#pragma unroll
+        for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[h][i])::"memory");
 }
+template <int N> struct Steps { static constexpr int value = N; };
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // SiLU with ONE SFU operation: x * sigmoid(x) = h + h * tanh(h), h = x / 2  (MUFU.TANH + 1 FMUL + 1 FFMA per element).
 // max |error| 1.0e-5 on [-12, 12] -- below fp16 output rounding for |x| > 0.02 and far below bf16's.
@@ -191,12 +211,14 @@ __device__ __forceinline__ void stage_box(const float (&acc)[BN / 2], int bx, co
 }
 
 template <bool F32, bool F16, int MT, int BN>
-__global__ void __launch_bounds__(256 * MT + 32 * kMaxProducers, (MT == 1 && BN <= 64) ? 2 : 1)
+__global__ void __launch_bounds__(conv_threads(MT), 1)
 conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                      const __grid_constant__ CUtensorMap map_c, const float* __restrict__ bias, int* __restrict__ sched,
                      const ConvParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
     constexpr int kConsumerWarps = 8 * MT;
+    constexpr bool kPingPong = ping_pong(MT, BN);
+    constexpr int kSlots = kPingPong ? 2 : MT;          // epilogue groups: staging boxes, named barrier, split-K flag each
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int a_bytes = kTileM * p.BK * 2;             // one sub-tile's A operand (generic / flat mode)
     const int b_bytes = BN * p.BK * 2;
@@ -209,14 +231,15 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
     constexpr int box_bytes = kTileM * 128;             // one staging box: 128 pixels x 128 B (64 halves / 32 floats of channels)
     const int staging_bytes = p.out_bufs * box_bytes;   // per sub-tile
     uint8_t* stage_out = ring + kStages * stage_bytes;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(stage_out + MT * staging_bytes);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(stage_out + kSlots * staging_bytes);
     uint64_t* empty_bar = full_bar + kMaxStages;
     uint64_t* ring_full = empty_bar + kMaxStages;                             // [kRing] tile-index ring, producer -> everybody else
     uint64_t* ring_empty = ring_full + kRing;                                 // [kRing]
     uint64_t* a_full = ring_empty + kRing;                                    // [kMaxHalo] halo-tile ring (halo mode)
     uint64_t* a_empty = a_full + kMaxHalo;
-    int* tile_ring = reinterpret_cast<int*>(a_empty + kMaxHalo);              // [kRing]
-    int* last_flag = tile_ring + kRing;                                       // [2] split-K: "this sub-tile's group reduces the tile"
+    uint64_t* mma_turn = a_empty + kMaxHalo;                                  // [2] ping-pong: "warpgroup w may issue its MMAs"
+    int* tile_ring = reinterpret_cast<int*>(mma_turn + 2);                    // [kRing]
+    int* last_flag = tile_ring + kRing;                                       // [2] split-K: "this epilogue group reduces the tile"
     int* first_unit = last_flag + 2;                                          // the CTA's first work unit (ticket drawn at entry)
 
     // generic mode walks K channel-chunk-major (step kt = chunk kt / taps, tap kt % taps), the order the halo mode accumulates in:
@@ -239,9 +262,12 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_c) : "memory");
-        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2 * MT); }   // released by every consumer warpgroup
+        // operand stages and halo buffers are released by every warpgroup that reads them: the owner alone in ping-pong
+        constexpr int readers = kPingPong ? 1 : 2 * MT;
+        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], readers); }
         for (int r = 0; r < kRing; ++r) { mbar_init(&ring_full[r], 1); mbar_init(&ring_empty[r], P - 1 + kConsumerWarps); }
-        for (int h = 0; h < kMaxHalo; ++h) { mbar_init(&a_full[h], 1); mbar_init(&a_empty[h], 2 * MT); }
+        for (int h = 0; h < kMaxHalo; ++h) { mbar_init(&a_full[h], 1); mbar_init(&a_empty[h], readers); }
+        for (int w = 0; w < 2; ++w) mbar_init(&mma_turn[w], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -274,6 +300,8 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
     };
 
     if (pw >= 0) {
+        setmaxnreg_dec<kProducerRegs>();    // the whole producer warpgroup, before any warp of it leaves
+        if (pw >= P) return;
         // ===== TMA producers.  Producer 0 is also the tile scheduler: the first unit is the ticket drawn at entry, later ones are drawn from
         // the same global counter, so a CTA that starts late (or shares its SM with another stream's kernel) simply takes fewer tiles
         // instead of stretching the layer; every unit index (and the final -1) is published to the other producer and the consumer
@@ -408,15 +436,21 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
             __threadfence();
         }
     } else {
-        // ===== consumers: sub-tile g = warps [8 g, 8 g + 8) = two warpgroups; warpgroup half hh owns pixel rows [64 hh, 64 hh + 64) of it.
+        // ===== consumers.  Ping-pong: warpgroup wg owns whole 128-pixel tiles (m64 halves 0 and 1) and takes ring entries wg, wg + 2, ...
+        // Cooperative: sub-tile g = warps [8 g, 8 g + 8) = two warpgroups; warpgroup half hh owns pixel rows [64 hh, 64 hh + 64) of it.
         // Each warpgroup issues its own wgmma chain into its registers and releases a ring stage (one arrival per warpgroup) once the
         // wgmmas that read it have retired: wait_group 1 after each stage's batch, so the tensor core always has the next batch queued.
-        const int g = warp >> 3;
-        const int hh = (warp >> 2) & 1;
-        const int gtid = (int)threadIdx.x - g * 256;      // thread index inside the sub-tile's group
-        const int bar_id = 1 + g;
+        setmaxnreg_inc<consumer_regs(MT)>();
+        constexpr int kHalves = kPingPong ? 2 : 1;                 // m64 halves per warpgroup
+        constexpr int kGroupThreads = kPingPong ? 128 : 256;      // threads that share an epilogue (one 128-pixel sub-tile)
+        const int wg = warp >> 2;
+        const int slot = kPingPong ? wg : warp >> 3;              // epilogue group: staging boxes, named barrier, split-K flag
+        const int g = kPingPong ? 0 : warp >> 3;                  // sub-tile
+        const int hh0 = kPingPong ? 0 : wg & 1;                   // first m64 half this warpgroup computes
+        const int gtid = (int)threadIdx.x - slot * kGroupThreads; // thread index inside the epilogue group
+        const int bar_id = 1 + slot;
         const bool wg_leader = (threadIdx.x & 127) == 0;
-        const int r0 = hh * 64 + (warp & 3) * 16 + (lane >> 2);      // this thread's first accumulator row inside the sub-tile (and r0 + 8)
+        const int rw = (warp & 3) * 16 + (lane >> 2);             // this thread's first accumulator row inside an m64 half (and rw + 8)
         // shared-memory matrix descriptor = {lo: (address >> 4) | LBO 1 << 16, hi: SBO >> 4 | swizzle mode << 30 (1 = 128 B, 2 = 64 B,
         // 3 = 32 B)}: K-major rows of BK*2 bytes, 8-row groups SBO bytes apart.  The swizzle is a function of the absolute shared-memory
         // address (the TMA unit writes the tiles the same way), so a start address shifted by whole rows and an SBO of any multiple of
@@ -431,10 +465,11 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
         const uint32_t stage_step = (uint32_t)stage_bytes >> 4, halo_step = (uint32_t)p.halo_bytes >> 4;
         const uint32_t b_off = (uint32_t)(MT * a_bytes) >> 4, b_step = (uint32_t)b_bytes >> 4;
         const uint32_t row_step = (uint32_t)row_bytes >> 4;        // halo windows shift by whole pixel rows of the tile
-        // this warpgroup's 64 rows: sub-tile g (sub_off), second half = 8 row groups further (8 tile rows of the halo tile, or 64 rows)
-        const uint32_t a_off = (uint32_t)(g * p.sub_off) / 16u + (uint32_t)hh * (p.halo ? 8u * (uint32_t)halo_w * row_step : 64u * row_step);
+        // the first half's rows: sub-tile g (sub_off), half hh0; the second half = 8 row groups further (8 tile rows of the halo tile, or 64 rows)
+        const uint32_t half_step = p.halo ? 8u * (uint32_t)halo_w * row_step : 64u * row_step;
+        const uint32_t a_off = (uint32_t)(g * p.sub_off) / 16u + (uint32_t)hh0 * half_step;
         auto desc = [](uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; };
-        const int ksub = p.BK / 16;
+        const int ksub = p.BK / 16;                       // k16 steps per K chunk: 4, 2 or 1
         bool b_ready = false;
         int stage = 0; uint32_t phase = 0;
         int hbuf = 0; uint32_t hphase = 0;
@@ -442,7 +477,11 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
         constexpr int cols_per_box = F32 ? 32 : 64;
         constexpr int nboxes = (BN + cols_per_box - 1) / cols_per_box;
         int box_seq = 0;                                  // running box counter: staging buffer = box_seq & 1 when there are two
-        float acc[BN / 2];
+        int entry = 0;                                    // ping-pong: ring entries seen (entry % 2 == wg: this warpgroup's tile)
+        int turns = 0;                                    // ping-pong: tiles this warpgroup has run
+        // ring position after n more steps of a ring of `len` slots
+        auto advance = [](int& pos, uint32_t& ph, int n, int len) { const int t = pos + n; ph ^= (uint32_t)((t / len) & 1); pos = t % len; };
+        float acc[kHalves][BN / 2];
         for (;;) {
             mbar_wait(&ring_full[rslot], rphase);
             const int u = tile_ring[rslot];
@@ -452,6 +491,19 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
             if (u < 0) break;
             int n0, img, ho0, wo0, k0, k1; long long pix0;
             unit_coords(u, n0, img, ho0, wo0, pix0, k0, k1);
+            if (kPingPong && (entry++ & 1) != wg) {
+                // the other warpgroup's tile: step over its operand stages and halo buffers in the shared rings
+                if (p.halo) {
+                    advance(hbuf, hphase, k1 - k0, p.halo_bufs);
+                    if (!p.b_res) advance(stage, phase, (k1 - k0) * (9 / p.tps), kStages);
+                } else {
+                    advance(stage, phase, k1 - k0, kStages);
+                }
+                continue;
+            }
+            // ping-pong hand-off: warpgroup 0's tile j waits until warpgroup 1 has issued the MMAs of its tile j - 1, warpgroup 1's
+            // tile j until warpgroup 0 has issued those of its tile j -- the MMA loops alternate, each epilogue runs under the other's MMAs
+            if (kPingPong && (wg == 1 || turns > 0)) mbar_wait(&mma_turn[wg], (uint32_t)((wg == 0 ? turns - 1 : turns) & 1));
             // ring stage / halo buffer read by the most recent committed batch: released once a later wait_group shows it retired
             int pend_stage = -1, pend_halo = -1;
             auto release = [&](int st, int hb) {
@@ -478,6 +530,22 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
                 }
             };
             uint32_t scale = 0;                             // the unit's first wgmma overwrites the accumulator
+            // one K chunk = BK / 16 k16 steps x the warpgroup's m64 halves.  The step count is made a compile-time constant so the chunk is
+            // ONE straight-line wgmma chain: in a runtime-count loop ptxas ends a wgmma group and injects a warpgroup.arrive every step.
+            auto chain = [&](auto ksteps, uint32_t a_lo, uint32_t b_lo) {
+#pragma unroll
+                for (int k = 0; k < decltype(ksteps)::value; ++k) {
+#pragma unroll
+                    for (int h = 0; h < kHalves; ++h)
+                        wgmma_m64k16<BN, F16>(acc[h], desc(a_lo + (uint32_t)h * half_step + 2u * k, hi_a), desc(b_lo + 2u * k, hi_b), scale);
+                    scale = 1;
+                }
+            };
+            auto mma_chunk = [&](uint32_t a_lo, uint32_t b_lo) {
+                if (ksub == 4) chain(Steps<4>{}, a_lo, b_lo);
+                else if (ksub == 2) chain(Steps<2>{}, a_lo, b_lo);
+                else chain(Steps<1>{}, a_lo, b_lo);
+            };
             if (p.halo) {
                 for (int kc = k0; kc < k1; ++kc) {
                     mbar_wait(&a_full[hbuf], hphase);
@@ -496,10 +564,7 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
                             const int tap = tap0 + t, kh = tap / 3, kw = tap - 3 * kh;
                             const uint32_t a_lo = a_buf + (uint32_t)(kh * halo_w + kw) * row_step;
                             const uint32_t b_lo = b_stage + (uint32_t)t * b_step;
-                            for (int k = 0; k < ksub; ++k) {
-                                wgmma_m64k16<BN, F16>(acc, desc(a_lo + 2u * k, hi_a), desc(b_lo + 2u * k, hi_b), scale);
-                                scale = 1;
-                            }
+                            mma_chunk(a_lo, b_lo);
                         }
                         wgmma_commit();
                         const bool chunk_end = tap0 + p.tps >= 9;
@@ -517,14 +582,15 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
                 wgmma_fence();
                 for (int j = 0; j < p.kpair; ++j) {       // K chunks of this stage: [chunk][sub-tile][128 rows] | [chunk][BN rows]
                     const uint32_t a_lo = a_st + (uint32_t)j * b_off + a_off, b_lo = b_st + (uint32_t)j * b_step;
-                    for (int k = 0; k < ksub; ++k) {
-                        wgmma_m64k16<BN, F16>(acc, desc(a_lo + 2u * k, hi_a), desc(b_lo + 2u * k, hi_b), scale);
-                        scale = 1;
-                    }
+                    mma_chunk(a_lo, b_lo);
                 }
                 wgmma_commit();
                 retire(stage, -1, kStages == 1);
                 if (++stage == kStages) { stage = 0; phase ^= 1; }
+            }
+            if (kPingPong) {                                // every MMA of this tile is issued: the other warpgroup's turn
+                if (wg_leader) mbar_arrive(&mma_turn[wg ^ 1]);
+                ++turns;
             }
             wgmma_wait<0>();
             acc_fence(acc);
@@ -541,35 +607,45 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
                 const int cq = 2 * (lane & 3);
                 float* wsub = p.ws + ((size_t)u * MT + g) * kTileM * BN;
 #pragma unroll
-                for (int j = 0; j < BN / 8; ++j)
+                for (int hf = 0; hf < kHalves; ++hf) {
+                    const int r0 = (hh0 + hf) * 64 + rw;
 #pragma unroll
-                    for (int h = 0; h < 2; ++h)
-                        __stcg(reinterpret_cast<float2*>(wsub + (size_t)(r0 + 8 * h) * BN + 8 * j + cq), make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]));
+                    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+                            __stcg(reinterpret_cast<float2*>(wsub + (size_t)(r0 + 8 * h) * BN + 8 * j + cq), make_float2(acc[hf][4 * j + 2 * h], acc[hf][4 * j + 2 * h + 1]));
+                }
                 __threadfence();
-                asm volatile("bar.sync %0, 256;" ::"r"(bar_id) : "memory");
+                asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "n"(kGroupThreads) : "memory");
                 if (gtid == 0) {
                     const int t = u / p.splits;
                     const int old = atomicAdd(p.flags + t * MT + g, 1);
                     const int last = old == p.splits - 1;
                     if (last) p.flags[t * MT + g] = 0;              // re-armed for the next launch
-                    last_flag[g] = last;
+                    last_flag[slot] = last;
                 }
-                asm volatile("bar.sync %0, 256;" ::"r"(bar_id) : "memory");
-                reduce_here = last_flag[g] != 0;
+                asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "n"(kGroupThreads) : "memory");
+                reduce_here = last_flag[slot] != 0;
                 if (reduce_here) {
                     __threadfence();
                     const int t = u / p.splits;
 #pragma unroll
-                    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+                    for (int hf = 0; hf < kHalves; ++hf)
+#pragma unroll
+                        for (int i = 0; i < BN / 2; ++i) acc[hf][i] = 0.f;
                     for (int sp = 0; sp < p.splits; ++sp) {
                         const float* src = p.ws + (((size_t)t * p.splits + sp) * MT + g) * kTileM * BN;
 #pragma unroll
-                        for (int j = 0; j < BN / 8; ++j)
+                        for (int hf = 0; hf < kHalves; ++hf) {
+                            const int r0 = (hh0 + hf) * 64 + rw;
 #pragma unroll
-                            for (int h = 0; h < 2; ++h) {
-                                const float2 x = __ldcg(reinterpret_cast<const float2*>(src + (size_t)(r0 + 8 * h) * BN + 8 * j + cq));
-                                acc[4 * j + 2 * h] += x.x; acc[4 * j + 2 * h + 1] += x.y;
-                            }
+                            for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                                for (int h = 0; h < 2; ++h) {
+                                    const float2 x = __ldcg(reinterpret_cast<const float2*>(src + (size_t)(r0 + 8 * h) * BN + 8 * j + cq));
+                                    acc[hf][4 * j + 2 * h] += x.x; acc[hf][4 * j + 2 * h + 1] += x.y;
+                                }
+                        }
                     }
                 }
             }
@@ -579,16 +655,20 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
                 const float* bias_t = bias + n0;
 #pragma unroll
                 for (int bx = 0; bx < nboxes; ++bx, ++box_seq) {
-                    uint8_t* stage_cur = stage_out + g * staging_bytes + (p.out_bufs == 2 ? (box_seq & 1) * box_bytes : 0);
+                    uint8_t* stage_cur = stage_out + slot * staging_bytes + (p.out_bufs == 2 ? (box_seq & 1) * box_bytes : 0);
                     // the store that used this buffer (out_bufs boxes ago) must have finished READING it
                     if (gtid == 0) {
                         if (p.out_bufs == 2) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
                         else asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
                     }
-                    asm volatile("bar.sync %0, 256;" ::"r"(bar_id) : "memory");
-                    if (in_range) stage_box<F32, F16, BN>(acc, bx, bias_t, stage_cur, r0, lane, p.act, p.act_floor, p.act_slope);
+                    asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "n"(kGroupThreads) : "memory");
+                    if (in_range) {
+#pragma unroll
+                        for (int hf = 0; hf < kHalves; ++hf)
+                            stage_box<F32, F16, BN>(acc[hf], bx, bias_t, stage_cur, (hh0 + hf) * 64 + rw, lane, p.act, p.act_floor, p.act_slope);
+                    }
                     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic-proxy writes -> visible to the TMA unit
-                    asm volatile("bar.sync %0, 256;" ::"r"(bar_id) : "memory");     // the eight warps of this sub-tile
+                    asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "n"(kGroupThreads) : "memory");   // the warps of this sub-tile
                     if (gtid == 0) {
                         const int cc = n0 + bx * cols_per_box;
                         if (in_range && cc < p.Cout) {
@@ -858,26 +938,24 @@ extern "C" int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_
     if (halo) { p.halo_bytes = ((p.TW * MT + 2) * (p.TH + 2) * bk * 2 + 1023) / 1024 * 1024; p.halo_bufs = 2; }
     const int box_bytes = kTileM * 128;                  // one staging box: 128 pixels x 64 halves / 32 floats
     p.out_bufs = d->out_bufs == 1 ? 1 : 2;
-    auto smem_for = [&](int st) { return (size_t)p.halo_bufs * p.halo_bytes + (size_t)st * stage_bytes + (size_t)MT * p.out_bufs * box_bytes + 512 + 1024; };
+    const int slots = ping_pong(MT, bn) ? 2 : MT;        // epilogue groups with their own staging boxes: warpgroups (ping-pong) or sub-tiles
+    auto smem_for = [&](int st) { return (size_t)p.halo_bufs * p.halo_bytes + (size_t)st * stage_bytes + (size_t)slots * p.out_bufs * box_bytes + 512 + 1024; };
     ConvKernelFn kfn = kernel_for(p.out_f32, p.f16, MT, bn);
     if (!kfn) { free_plan(pl); return cfail(B2T_EINVAL, "b2t_conv_plan_create: no kernel for this mt / BLOCK_N"); }
     // the opt-in for > 48 KB of dynamic shared memory is per device and per kernel instantiation
     if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
         free_plan(pl); return cfail(B2T_ECUDA, "cannot raise dynamic shared memory for conv kernel");
     }
-    cudaFuncAttributes fa;
-    if (cudaFuncGetAttributes(&fa, kfn) != cudaSuccess) { free_plan(pl); return cfail(B2T_ECUDA, "cudaFuncGetAttributes(conv kernel) failed"); }
-    // Ring depth: what bounds a CTA is the data it keeps in flight, so by default the ring takes the shared memory that is left --
-    // up to kMaxStages -- after deciding how many CTAs share the SM: 2 when their registers and >= 3 stages each fit, else 1.
-    const bool two_by_regs = 2 * fa.numRegs * (256 * MT + 32 * kMaxProducers) <= 65536;
+    // Ring depth: what bounds a CTA is the data it keeps in flight, so by default the ring takes the shared memory that is left, up to
+    // kMaxStages.  The register hand-off sizes every instantiation for one CTA per SM (its launch allocation is the whole register file).
+    const int threads = conv_threads(MT);                // consumer warpgroups + the producer warpgroup, whatever P is
     int stages = d->stages > 0 ? (d->stages < kMaxStages ? d->stages : kMaxStages) : 0;
     if (p.b_res) stages = 1;
     const int min_stages = (halo || p.kpair == 2) ? 2 : 3;
     if (stages == 0) {
         for (int pass = 0; pass < 2 && stages == 0; ++pass) {
-            int per2 = 0, per1 = 0;
-            for (int st = kMaxStages; st >= 1; --st) { if (!per2 && smem_for(st) <= 113 * 1024) per2 = st; if (!per1 && smem_for(st) <= 226 * 1024) per1 = st; }
-            const int pick = (two_by_regs && MT == 1 && per2 >= 3) ? per2 : per1;
+            int pick = 0;
+            for (int st = kMaxStages; st >= 1 && !pick; --st) if (smem_for(st) <= 226 * 1024) pick = st;
             if (pick >= min_stages || p.out_bufs == 1 || d->out_bufs == 2) stages = pick;
             else p.out_bufs = 1;                          // a second staging box is worth less than a ring stage
         }
@@ -891,7 +969,6 @@ extern "C" int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_
     // producers it could run two phases ahead of a stage and alias it -- never more producers than stages
     const int P_eff = P > stages ? stages : P;
     p.P = P_eff;
-    const int threads = 256 * MT + 32 * P_eff;
     p.stages = stages;
     pl->smem = smem_for(stages);
     pl->threads = threads;
@@ -937,9 +1014,9 @@ extern "C" double b2t_conv_plan_flops(const b2t_conv_plan* pl) { return pl ? pl-
 extern "C" int b2t_conv_plan_info(const b2t_conv_plan* pl, int* out, int n) {
     if (!pl || !out) return cfail(B2T_EINVAL, "b2t_conv_plan_info: null argument");
     const ConvParams& p = pl->p;
-    const int v[17] = {(int)pl->grid.x, pl->threads, (int)pl->smem, p.BN, p.stages, p.MT, p.splits, p.halo, p.halo_bufs, p.tiles_m, p.tiles_n, p.BN / 2, p.P,
-                       p.tps, p.b_res, p.out_bufs, p.kpair};
-    for (int i = 0; i < n && i < 17; ++i) out[i] = v[i];
+    const int v[18] = {(int)pl->grid.x, pl->threads, (int)pl->smem, p.BN, p.stages, p.MT, p.splits, p.halo, p.halo_bufs, p.tiles_m, p.tiles_n,
+                       p.BN / 2 * (ping_pong(p.MT, p.BN) ? 2 : 1), p.P, p.tps, p.b_res, p.out_bufs, p.kpair, ping_pong(p.MT, p.BN) ? 1 : 0};
+    for (int i = 0; i < n && i < 18; ++i) out[i] = v[i];
     return B2T_OK;
 }
 
