@@ -95,6 +95,12 @@ typedef struct b2t_tracker_config {
     double conf_thresh; /* opts.conf_thresh (basetrack.py:354), a Python float in the reference */
     double iou_thresh;  /* opts.iou_thresh, SORT only (basetrack.py:414,438) */
     double frame_rate;  /* tracker ctor frame_rate */
+    /* BoT-SORT with ReID (use_apperance_model, botsort.py:345-349, :386-392, :440-446), B2T_BOTSORT only.  0 = off: the state
+     * size and every result are those of a tracker without the fields.  Otherwise the length of the appearance features, a
+     * multiple of 32 up to 2048; the state block then holds each track's smoothed feature, feat [S][cap][feat_dim] float32. */
+    int feat_dim;
+    double theta_iou;   /* associations 1 and 3: the appearance cost counts only where the IoU distance is <= theta_iou (< 1) ... */
+    double theta_emb;   /* ... and 0.5 (1 - cos) is <= theta_emb; cost = min(IoU distance, appearance cost).  Defaults 0.5 / 0.25 */
 } b2t_tracker_config;
 
 size_t b2t_tracker_state_bytes(const b2t_tracker_config* cfg);
@@ -103,7 +109,9 @@ int b2t_tracker_create(const b2t_tracker_config* cfg, void* state_mem, void* str
 int b2t_tracker_reset(b2t_tracker* t, void* stream);
 void b2t_tracker_destroy(b2t_tracker* t);
 int b2t_tracker_out_cols(void);   /* 8: id, x, y, w, h, cls, score, slot */
-int b2t_tracker_stat_words(void); /* 64: [0..16) counters, [16..32) per-phase SM cycles, [32..64) sub-phase cycles */
+/* 64: [0..16) counters, [16..29) per-phase SM cycles, [30] pairs of associations 1 and 3 given an appearance cost, [31] pairs whose
+ * cost the appearance lowered (both 0 without features), [32..64) sub-phase cycles */
+int b2t_tracker_stat_words(void);
 /* One frame for every sequence.
  *   dets      [S][dmax][6] float32  x1,y1,x2,y2,score,cls (what track.py:149 hands to tracker.update)
  *             a box the reference cannot track is ignored (a deliberate divergence): a non-finite coordinate, y2 == y1, or
@@ -112,9 +120,21 @@ int b2t_tracker_stat_words(void); /* 64: [0..16) counters, [16..32) per-phase SM
  *   warps     [S][6] float64 or NULL (BoT-SORT camera motion, botsort.py:380)
  *   id_base   [S] int32 or NULL: overrides the sequence's id counter before births (BaseTrack._count)
  *   out       [S][out_rows][8] float64, stat [S][64] int32
- *   predict_only != 0 -> update_without_detection (basetrack.py:489-537) */
+ *   predict_only != 0 -> update_without_detection (basetrack.py:489-537)
+ * B2T_EINVAL on a tracker with feat_dim > 0. */
 int b2t_tracker_step(b2t_tracker* t, const float* dets, const int* det_count, const double* warps,
                      const int* id_base, double* out, int out_rows, int* stat, int predict_only, void* stream);
+/* The same step for a tracker with feat_dim > 0 (B2T_EINVAL otherwise).  feats [S][dmax][feat_dim] float32, 16-B aligned: row i
+ * is the appearance feature of detection row i, as the extractor returned it (not re-normalised).  Only the rows with
+ * score >= conf_thresh are read; NULL is allowed with predict_only.  Associations 1 and 3 fuse the appearance cost; a track
+ * updated by a high-score detection smooths its feature (STrack.update, basetrack.py:323-332, float32); a birth stores the
+ * detection's feature; re-activation and low-score updates leave it unchanged. */
+int b2t_tracker_step_feat(b2t_tracker* t, const float* dets, const int* det_count, const float* feats, const double* warps,
+                          const int* id_base, double* out, int out_rows, int* stat, int predict_only, void* stream);
+/* Changes theta_iou / theta_emb for the following steps (the reference reads them as plain attributes every frame). */
+int b2t_tracker_set_thetas(b2t_tracker* t, double theta_iou, double theta_emb);
+/* Copies one slot's smoothed feature (feat_dim floats) to the HOST (lazy STrack.features).  Synchronises the stream. */
+int b2t_tracker_read_feature(b2t_tracker* t, int seq, int slot, float* host, void* stream);
 /* Same with HOST buffers (pinned recommended); device staging lives inside the state block. */
 int b2t_tracker_step_host(b2t_tracker* t, const float* dets_host, const int* det_count_host,
                           const double* warps_host, const int* id_base_host, double* out_host, int out_rows,

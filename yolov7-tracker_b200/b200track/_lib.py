@@ -16,6 +16,7 @@ SORT, BYTETRACK, BOTSORT = 0, 1, 2
 FLAG_MEAN_F32, FLAG_NOT_TRACKED = 1, 2
 ACT_BF16, ACT_F16 = 0, 1
 OUT_COLS, STAT_WORDS, STAT_PHASE0, STAT_SUB0 = 8, 64, 16, 32
+STAT_NAPP, STAT_NAPPLOW = 30, 31          # appearance pairs, and those whose cost the appearance lowered
 GMC_STAT_WORDS, GMC_FIRST_FRAME, GMC_FEW_POINTS, GMC_TRUNCATED = 8, 1, 2, 4
 (STAT_NOUT, STAT_NEXT_ID, STAT_NTRACKED, STAT_NLOST, STAT_ERR, STAT_FRAME, STAT_NPOOL, STAT_NBIRTH,
  STAT_NHI, STAT_NLO, STAT_NEDGE, STAT_NMATCH0) = range(12)
@@ -30,7 +31,8 @@ class B2TError(RuntimeError):
 class TrackerConfig(C.Structure):
     _fields_ = [("kind", C.c_int), ("dtype", C.c_int), ("fmt", C.c_int), ("n_seq", C.c_int), ("cap", C.c_int),
                 ("dmax", C.c_int), ("ecap", C.c_int), ("use_gmc", C.c_int), ("track_buffer", C.c_int),
-                ("conf_thresh", C.c_double), ("iou_thresh", C.c_double), ("frame_rate", C.c_double)]
+                ("conf_thresh", C.c_double), ("iou_thresh", C.c_double), ("frame_rate", C.c_double),
+                ("feat_dim", C.c_int), ("theta_iou", C.c_double), ("theta_emb", C.c_double)]
 
 
 class ConvDesc(C.Structure):
@@ -65,6 +67,9 @@ SIGNATURES = {
     "b2t_tracker_stat_words": (_I, []),
     "b2t_tracker_step": (_I, [_P, _P, _P, _P, _P, _P, _I, _P, _I, _P]),
     "b2t_tracker_step_host": (_I, [_P, _P, _P, _P, _P, _P, _I, _P, _I, _P]),
+    "b2t_tracker_step_feat": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _P, _I, _P]),
+    "b2t_tracker_set_thetas": (_I, [_P, _D, _D]),
+    "b2t_tracker_read_feature": (_I, [_P, _I, _I, _P, _P]),
     "b2t_tracker_read_slot": (_I, [_P, _I, _I, _P, _P, _P]),
     "b2t_tracker_list_cols": (_I, []),
     "b2t_tracker_read_list": (_I, [_P, _I, _I, _P, _I, C.POINTER(C.c_int), _P]),

@@ -18,7 +18,11 @@ def _dev_ptr(t):
 
 class TrackEngine:
     def __init__(self, kind="bytetrack", n_seq=1, dtype="f64", cap=1024, dmax=1024, ecap=None, kalman_format=None,
-                 conf_thresh=0.2, iou_thresh=0.5, track_buffer=30, frame_rate=30, use_gmc=True, device="cuda:0"):
+                 conf_thresh=0.2, iou_thresh=0.5, track_buffer=30, frame_rate=30, use_gmc=True, device="cuda:0",
+                 feat_dim=0, theta_iou=0.5, theta_emb=0.25):
+        """feat_dim > 0 (BoT-SORT only, a multiple of 32 up to 2048): BoT-SORT with appearance features -- every step then takes the
+        detections' features (step_device(feats=), step_cuda_dets(feats_list=)) and fuses them into associations 1 and 3 with the
+        gates theta_iou / theta_emb (set_thetas changes them between steps)."""
         if not torch.cuda.is_available():
             raise L.B2TError("TrackEngine needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.lib = L.load()
@@ -32,10 +36,12 @@ class TrackEngine:
         if ecap is None:
             ecap = 128 * max(cap, dmax)       # sub-threshold (track, detection) pairs per association: 2 MB of spill per sequence
         self.S, self.cap, self.dmax, self.ecap = n_seq, cap, dmax, ecap
+        self.feat_dim, self.theta_iou, self.theta_emb = int(feat_dim), float(theta_iou), float(theta_emb)
         self.cfg = L.TrackerConfig(kind=L.KIND_BY_NAME[kind], dtype=self.dtype, fmt=L.FMT_BY_NAME[kalman_format],
                                    n_seq=n_seq, cap=cap, dmax=dmax, ecap=ecap, use_gmc=int(bool(use_gmc)),
                                    track_buffer=int(track_buffer), conf_thresh=float(conf_thresh),
-                                   iou_thresh=float(iou_thresh), frame_rate=float(frame_rate))
+                                   iou_thresh=float(iou_thresh), frame_rate=float(frame_rate), feat_dim=self.feat_dim,
+                                   theta_iou=self.theta_iou, theta_emb=self.theta_emb)
         nbytes = self.lib.b2t_tracker_state_bytes(C.byref(self.cfg))
         if nbytes == 0:
             raise L.B2TError((self.lib.b2t_last_error() or b"").decode())
@@ -70,6 +76,12 @@ class TrackEngine:
                 self.handle = None
         except Exception:
             pass
+
+    def set_thetas(self, theta_iou, theta_emb):
+        """BoT-SORT's appearance gates for the following steps (b2t_tracker_set_thetas); theta_iou < 1."""
+        if (float(theta_iou), float(theta_emb)) != (self.theta_iou, self.theta_emb):
+            L.check(self.lib, self.lib.b2t_tracker_set_thetas(self.handle, float(theta_iou), float(theta_emb)))
+            self.theta_iou, self.theta_emb = float(theta_iou), float(theta_emb)
 
     def reset(self):
         L.check(self.lib, self.lib.b2t_tracker_reset(self.handle, self._stream()))
@@ -107,12 +119,14 @@ class TrackEngine:
         self.d2h_bytes_per_step = self.S * (self.out_rows * L.OUT_COLS * 8 + L.STAT_WORDS * 4)
         return self.results()
 
-    def step_cuda_dets(self, dets_list, warps=None, id_base=None):
+    def step_cuda_dets(self, dets_list, warps=None, id_base=None, feats_list=None, predict_only=False):
         """Detections that already live on THIS device (the NMS output tracker/track.py:151 hands to tracker.update): no host round
         trip of the boxes.  dets_list: per sequence an (n_i, 6) float32 CUDA tensor.  The rows are copied device-to-device into the
         kernel's [sequence][dmax][6] layout, the counts / id base / warps (a few bytes) go up from pinned memory, the fused kernel
         runs, track rows + stats come back asynchronously and ONE stream synchronisation ends the call (the API returns Python
-        objects).  Same results as step(); 24 B + 24 KB... less traffic and one sync instead of three."""
+        objects).  Same results as step(); 24 B + 24 KB... less traffic and one sync instead of three.
+        feats_list (feat_dim > 0): per sequence an (n_i, feat_dim) float32 CUDA tensor of the detections' features, row-aligned with
+        dets_list (only the high-score rows are read)."""
         if not hasattr(self, "d_dets"):
             self.d_dets = torch.zeros((self.S, self.dmax, 6), dtype=torch.float32, device=self.device)
             self.d_count = torch.zeros(self.S, dtype=torch.int32, device=self.device)
@@ -120,6 +134,9 @@ class TrackEngine:
             self.d_warps = torch.zeros((self.S, 6), dtype=torch.float64, device=self.device)
             self.d_out = torch.zeros((self.S, self.cap, L.OUT_COLS), dtype=torch.float64, device=self.device)
             self.d_stat = torch.zeros((self.S, L.STAT_WORDS), dtype=torch.int32, device=self.device)
+            self.d_feats = torch.zeros((self.S, self.dmax, self.feat_dim), dtype=torch.float32, device=self.device) if self.feat_dim else None
+        if (feats_list is not None) != (self.feat_dim > 0) and not predict_only:
+            raise L.B2TError("step_cuda_dets: feats_list is required exactly when the engine has feat_dim > 0 (feat_dim = %d)" % self.feat_dim)
         for s, d in enumerate(dets_list):
             n = int(d.shape[0])
             if n > self.dmax:
@@ -128,6 +145,12 @@ class TrackEngine:
                 raise L.B2TError("step_cuda_dets: detections live on %s, the engine on %s" % (d.device, self.device))
             if n:
                 self.d_dets[s, :n].copy_(d.detach().reshape(n, 6).to(torch.float32), non_blocking=True)
+                if feats_list is not None:
+                    fe = feats_list[s]
+                    if tuple(fe.shape) != (n, self.feat_dim) or fe.device != self.device:
+                        raise L.B2TError("step_cuda_dets: sequence %d: features must be (%d, %d) on %s, got %s on %s"
+                                         % (s, n, self.feat_dim, self.device, tuple(fe.shape), fe.device))
+                    self.d_feats[s, :n].copy_(fe.detach().to(torch.float32), non_blocking=True)
             self.np_count[s] = n
         self.d_count.copy_(self.h_count, non_blocking=True)
         w = ib = None
@@ -141,7 +164,8 @@ class TrackEngine:
             ib = self.d_idbase
         rows = self.out_rows
         out = self.d_out[:, :rows] if rows == self.cap else self.d_out.view(-1)[: self.S * rows * L.OUT_COLS].view(self.S, rows, L.OUT_COLS)
-        self.step_device(self.d_dets, self.d_count, out, self.d_stat, warps=w, id_base=ib)
+        self.step_device(self.d_dets, self.d_count, out, self.d_stat, warps=w, id_base=ib,
+                         feats=self.d_feats if self.feat_dim else None, predict_only=predict_only)
         self.h_out.view(-1)[: self.S * rows * L.OUT_COLS].copy_(out.reshape(-1), non_blocking=True)
         self.h_stat.copy_(self.d_stat, non_blocking=True)
         torch.cuda.current_stream(self.device).synchronize()
@@ -160,9 +184,11 @@ class TrackEngine:
         return self.step_host(warps, id_base, predict_only)
 
     # ---- device-pointer path: detections already resident (detector output), no sync
-    def step_device(self, dets, det_count, out, stat, warps=None, id_base=None, predict_only=False):
+    def step_device(self, dets, det_count, out, stat, warps=None, id_base=None, predict_only=False, feats=None):
         """dets (S,dmax,6) f32, det_count (S) i32, out (S,rows,8) f64, stat (S,64) i32: contiguous CUDA tensors on this engine's
-        device.  The kernel indexes them as raw [sequence][dmax][6] / [sequence][rows][8] arrays: the layout is checked here."""
+        device.  The kernel indexes them as raw [sequence][dmax][6] / [sequence][rows][8] arrays: the layout is checked here.
+        feats (S,dmax,feat_dim) f32, row-aligned with dets: given, the step runs b2t_tracker_step_feat (the engine must have
+        feat_dim > 0, else the library refuses), otherwise b2t_tracker_step."""
         def _chk(t, shape, dtype, what):
             if t is None:
                 return
@@ -177,10 +203,17 @@ class TrackEngine:
         _chk(stat, (self.S, L.STAT_WORDS), torch.int32, "stat")
         _chk(warps, (self.S, 6), torch.float64, "warps")
         _chk(id_base, (self.S,), torch.int32, "id_base")
+        if feats is not None:
+            _chk(feats, (self.S, self.dmax, self.feat_dim), torch.float32, "feats")
         with torch.cuda.device(self.device):
-            rc = self.lib.b2t_tracker_step(self.handle, _dev_ptr(dets), _dev_ptr(det_count), _dev_ptr(warps),
-                                           _dev_ptr(id_base), _dev_ptr(out), int(out.shape[1]), _dev_ptr(stat),
-                                           int(predict_only), self._stream())
+            if feats is not None or (self.feat_dim and predict_only):
+                rc = self.lib.b2t_tracker_step_feat(self.handle, _dev_ptr(dets), _dev_ptr(det_count), _dev_ptr(feats), _dev_ptr(warps),
+                                                    _dev_ptr(id_base), _dev_ptr(out), int(out.shape[1]), _dev_ptr(stat),
+                                                    int(predict_only), self._stream())
+            else:
+                rc = self.lib.b2t_tracker_step(self.handle, _dev_ptr(dets), _dev_ptr(det_count), _dev_ptr(warps),
+                                               _dev_ptr(id_base), _dev_ptr(out), int(out.shape[1]), _dev_ptr(stat),
+                                               int(predict_only), self._stream())
         L.check(self.lib, rc)
 
     def read_list(self, seq, which="tracked"):
@@ -193,6 +226,14 @@ class TrackEngine:
                                                 C.byref(n), self._stream())
         L.check(self.lib, rc)
         return rows[:n.value].copy()
+
+    def read_feature(self, seq, slot):
+        """(feat_dim,) float32: the smoothed appearance feature of one slot (b2t_tracker_read_feature)."""
+        v = np.zeros(self.feat_dim, np.float32)
+        with torch.cuda.device(self.device):
+            rc = self.lib.b2t_tracker_read_feature(self.handle, int(seq), int(slot), v.ctypes.data_as(C.c_void_p), self._stream())
+        L.check(self.lib, rc)
+        return v
 
     def read_slot(self, seq, slot):
         mean = np.zeros(8); cov = np.zeros((8, 8))

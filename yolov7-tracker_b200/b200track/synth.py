@@ -54,6 +54,65 @@ def make_stream(seed, n_frames, n_obj=300, img=1280, miss=0.05, warp_sigma=0.0):
     return frames, warps
 
 
+def make_reid_stream(seed, n_frames, n_obj=60, feat_dim=64, img=1280, warp_sigma=1.0, occl=0.04):
+    """A stream for BoT-SORT with appearance features: (frames, feats, warps).  feats[f] is an (n_i, feat_dim) float32 array aligned
+    with the rows of frames[f] (the tracker reads only those of the high-score rows).
+      * half of the objects move in pairs that cross each other head-on at the same height, so IoU alone can swap them;
+      * every object has a seeded identity vector; a detection's feature is that vector plus noise, times a random scale in
+        [0.3, 3] -- the extractor's features are not assumed to be unit vectors;
+      * an object goes unseen for 3-8 frames with probability `occl` per frame (Lost tracks that are re-activated later);
+      * about 15 % of the detections score in [0.1, 0.2) (low-score association, no feature).
+    Coordinates are not rounded, so no two costs tie exactly."""
+    rng = np.random.default_rng(seed)
+    n_pair = n_obj // 4
+    cx = rng.uniform(150, img - 150, n_obj)
+    cy = rng.uniform(150, img - 150, n_obj)
+    w = rng.uniform(30, 70, n_obj)
+    h = rng.uniform(60, 140, n_obj)
+    vx = rng.normal(0, 1.5, n_obj)
+    vy = rng.normal(0, 1.5, n_obj)
+    for k in range(n_pair):                                   # objects 2k and 2k+1 cross half-way through the stream
+        a, b = 2 * k, 2 * k + 1
+        speed = rng.uniform(2.0, 5.0)
+        mid = rng.uniform(300, img - 300)
+        cx[a], cx[b] = mid - speed * n_frames / 2, mid + speed * n_frames / 2
+        cy[b] = cy[a] + rng.normal(0, 3)
+        vx[a], vx[b], vy[a], vy[b] = speed, -speed, 0.0, 0.0
+        w[b], h[b] = w[a] * rng.uniform(0.9, 1.1), h[a] * rng.uniform(0.9, 1.1)
+    ident = rng.normal(0, 1, (n_obj, feat_dim))
+    base_score = rng.uniform(0.35, 0.95, n_obj)
+    hidden = np.zeros(n_obj, np.int64)
+    frames, feats = [], []
+    warps = np.zeros((n_frames, 2, 3), dtype=np.float64)
+    warps[:, 0, 0] = warps[:, 1, 1] = 1.0
+    cam = np.zeros(2)
+    for f in range(n_frames):
+        cx += vx
+        cy += vy
+        t = rng.normal(0, warp_sigma, 2)
+        warps[f, :, 2] = t
+        cam += t
+        start = (hidden == 0) & (rng.uniform(0, 1, n_obj) < occl)
+        hidden[start] = rng.integers(3, 9, int(start.sum()))
+        seen = hidden == 0
+        hidden[~seen] -= 1
+        jit = rng.normal(0, 1.0, (n_obj, 4))
+        score = np.where(rng.uniform(0, 1, n_obj) < 0.15, rng.uniform(0.1, 0.2, n_obj), base_score + rng.normal(0, 0.02, n_obj))
+        x1 = cx - w / 2 + jit[:, 0] + cam[0]
+        y1 = cy - h / 2 + jit[:, 1] + cam[1]
+        x2 = cx + w / 2 + jit[:, 2] + cam[0]
+        y2 = cy + h / 2 + jit[:, 3] + cam[1]
+        box = np.clip(np.stack([x1, y1, x2, y2], 1), 0, img)
+        ok = seen & ((box[:, 2] - box[:, 0]) >= 4) & ((box[:, 3] - box[:, 1]) >= 4)
+        d = np.concatenate([box[ok], score[ok, None], (np.arange(n_obj) % 3)[ok, None]], 1).astype(np.float32)
+        fe = (ident[ok] + rng.normal(0, 0.6, (int(ok.sum()), feat_dim))) * rng.uniform(0.3, 3.0, (int(ok.sum()), 1))
+        fe = fe.astype(np.float32)
+        order = np.argsort(-d[:, 4], kind="stable")
+        frames.append(np.ascontiguousarray(d[order]))
+        feats.append(np.ascontiguousarray(fe[order]))
+    return frames, feats, warps
+
+
 def stream_digest(frames):
     """sha1 of the raw bytes: stored with golden fixtures to detect generator drift."""
     hsh = hashlib.sha1()

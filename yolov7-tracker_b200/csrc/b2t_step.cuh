@@ -15,6 +15,8 @@
 //   tracked/lost/freelist [S][cap] int32            ordered slot lists (order defines row order, q13)
 //   ctrl [S][16] int32                              frame, next_id, list lengths, error
 //   e_col [S][ecap] int32, e_cost [S][ecap] T       CSR edges of the current association
+//   feat [S][cap][feat_dim] float32, e_app [S][ecap] int32   BoT-SORT with ReID only (feat_dim > 0): each track's smoothed
+//                                                   appearance feature, and the edges of an association that get an appearance cost
 // Everything else (boxes, lists, assignment state) lives in shared memory for the frame.
 #pragma once
 #include "b2t_prims.cuh"
@@ -29,7 +31,9 @@ enum { ST_NEW = 0, ST_TRACKED = 1, ST_LOST = 2, ST_REMOVED = 3 };
 enum { CTRL_FRAME = 0, CTRL_NEXT_ID = 1, CTRL_NTRACKED = 2, CTRL_NLOST = 3, CTRL_NFREE = 4, CTRL_ERR = 5 };
 enum { STAT_NOUT = 0, STAT_NEXT_ID = 1, STAT_NTRACKED = 2, STAT_NLOST = 3, STAT_ERR = 4, STAT_FRAME = 5,
        STAT_NPOOL = 6, STAT_NBIRTH = 7, STAT_NHI = 8, STAT_NLO = 9, STAT_NEDGE = 10, STAT_NMATCH0 = 11,
-       STAT_PHASE0 = 16,   // [16..32): SM cycles spent per phase (thread 0's clock64 deltas)
+       STAT_PHASE0 = 16,   // [16..29): SM cycles spent per phase (thread 0's clock64 deltas)
+       STAT_NAPP = 30,     // pairs of associations 1 and 3 given an appearance cost (IoU distance <= theta_iou)
+       STAT_NAPPLOW = 31,  // ... of which the appearance cost was the lower one
        STAT_SUB0 = 32,     // [32..64): sub-phase cycle stamps of association 1 (CSR build, LAP)
        STAT_WORDS = 64 };
 enum { ERR_SLOTS = 1, ERR_EDGES = 2, ERR_DETS = 4, ERR_OUT = 8 };    // ERR_OUT: more confirmed tracks than output rows (rows were dropped)
@@ -43,6 +47,7 @@ struct TrackState {
     float *cls, *score;
     int *tracked, *lost, *freelist, *ctrl;
     int *e_col, *e_row; void* e_cost;
+    int feat_dim; float* feat; int* e_app;      // feat_dim == 0: no appearance state (feat, e_app null)
 };
 
 struct StepParams {
@@ -52,6 +57,7 @@ struct StepParams {
     int max_time_lost;
     int use_gmc;
     int predict_only;                           // update_without_detection (basetrack.py:489-537)
+    double theta_iou, theta_emb;                // BoT-SORT appearance gates (botsort.py:289), used with feat_dim > 0
 };
 
 template <class T> struct StepSmem {
@@ -120,10 +126,13 @@ template <class T> struct SeqView {
     int *tid, *state, *activated, *tracklet_len, *start_frame, *frame_id, *flags, *removed_at;
     float *cls, *score;
     int *tracked, *lost, *freelist, *ctrl, *e_col, *e_row;
-    int cap, ecap;
+    float* feat; int* e_app;
+    int cap, ecap, feat_dim;
     B2T_DEV SeqView(const TrackState& st, int s) {
         const size_t c = (size_t)st.cap, o = (size_t)s * c;
-        cap = st.cap; ecap = st.ecap;
+        cap = st.cap; ecap = st.ecap; feat_dim = st.feat_dim;
+        feat = st.feat ? st.feat + o * st.feat_dim : nullptr;
+        e_app = st.e_app ? st.e_app + (size_t)s * st.ecap : nullptr;
         mean = (T*)st.mean + o * 8; cov = (T*)st.cov + o * 64;
         tid = st.tid + o; state = st.state + o; activated = st.activated + o; tracklet_len = st.tracklet_len + o;
         start_frame = st.start_frame + o; frame_id = st.frame_id + o; flags = st.flags + o; removed_at = st.removed_at + o;
@@ -154,15 +163,65 @@ template <class T> B2T_DEV void fill_track_boxes(const SeqView<T>& v, int fmt, c
 //      holes (col = -1) that every consumer skips;
 //   3. rows whose range ends below esm live in shared memory, the others in the sequence's global
 //      edge workspace (same indices) -- LapCsr::cols/costs picks per row.
+//   With an appearance context (BoT-SORT with ReID, associations 1 and 3, botsort.py:386-392 / :440-446) the pairs whose IoU
+//   distance is <= theta_iou are listed in v.e_app, and one WARP per listed pair computes
+//   App = 0.5 (1 - cos) from the two feature rows (128-bit loads, a.b / a.a / b.b accumulated in T, shuffle reduction), masks
+//   App > theta_emb to 1 and keeps min(IoU distance, App).  Every other pair has App = 1, so its cost stays the IoU distance, and
+//   with theta_iou < 1 a non-overlapping pair (IoU distance 1) stays out: the candidate set is unchanged.
 // Requires m <= 1024.  Returns false (uniformly) on edge-workspace overflow.
+struct AppCtx {
+    const int* row_slot;    // [n] track slot of each row (its feature is v.feat[slot])
+    const int* col_det;     // [m] detection row of each column (its feature is feats[det])
+    const float* feats;     // this sequence's [dmax][feat_dim] detection features
+    double theta_iou, theta_emb;
+};
+
+// Stage 2b of build_csr: one warp per listed edge (list[q] = edge index, top bit set when the edge lives in the global workspace
+// g_* rather than in the shared-memory mirror s_*).  The edge holds its IoU distance; it receives min(IoU distance, App) or
+// becomes a hole.  Returns, on lane 0 of each warp, how many of its edges the appearance cost lowered.
 template <class T>
-B2T_DEVNI bool build_csr(SeqView<T>& v, StepSmem<T>& sm, int n, int m, T thresh, int* dbg = nullptr, long long* dbgt = nullptr) {
+B2T_DEVNI int app_costs(const AppCtx app, const float* tfeat, int D, const int* list, int na, int* s_col, const int* s_row,
+                        T* s_cost, int* g_col, const int* g_row, T* g_cost, T thresh) {
+    const int D4 = D >> 2, lane = lane_id();
+    const T th_emb = (T)app.theta_emb;
+    int lowered = 0;
+    for (int q = warp_id(); q < na; q += num_warps()) {
+        const int code = list[q], e = code & 0x7fffffff;
+        const bool glob = code < 0;
+        int* pc = glob ? g_col : s_col;
+        T* pw = glob ? g_cost : s_cost;
+        const int i = glob ? g_row[e] : s_row[e], j = pc[e];
+        const float4* a = reinterpret_cast<const float4*>(tfeat + (size_t)app.row_slot[i] * D);
+        const float4* b = reinterpret_cast<const float4*>(app.feats + (size_t)app.col_det[j] * D);
+        T ab = (T)0, aa = (T)0, bb = (T)0;
+        for (int k = lane; k < D4; k += 32) {
+            const float4 x = a[k], y = b[k];
+            ab += (T)x.x * (T)y.x + (T)x.y * (T)y.y + (T)x.z * (T)y.z + (T)x.w * (T)y.w;
+            aa += (T)x.x * (T)x.x + (T)x.y * (T)x.y + (T)x.z * (T)x.z + (T)x.w * (T)x.w;
+            bb += (T)y.x * (T)y.x + (T)y.y * (T)y.y + (T)y.z * (T)y.z + (T)y.w * (T)y.w;
+        }
+        for (int o = 16; o; o >>= 1) { ab += shfl_xor(ab, o); aa += shfl_xor(aa, o); bb += shfl_xor(bb, o); }
+        if (lane == 0) {
+            const T iou_d = pw[e];
+            T app_d = (T)0.5 * ((T)1 - ab / (sqrt(aa) * sqrt(bb)));    // 0.5 * matching.embedding_distance (cosine of the unit rows)
+            if (app_d > th_emb) app_d = (T)1;
+            const T dist = app_d < iou_d ? app_d : iou_d;
+            lowered += app_d < iou_d ? 1 : 0;
+            if (dist < thresh) pw[e] = dist; else pc[e] = -1;
+        }
+    }
+    return lowered;
+}
+
+template <class T>
+B2T_DEVNI bool build_csr(SeqView<T>& v, StepSmem<T>& sm, int n, int m, T thresh, int* dbg = nullptr, long long* dbgt = nullptr,
+                         const AppCtx* app = nullptr) {
     const int tid = (int)threadIdx.x, nthr = (int)blockDim.x, lane = lane_id();
     int* misc = sm.misc;
     const T* colbox = sm.colbox;
     const bool sorted = m > 64;
     T xmin = (T)0, scale = (T)0, maxw = (T)0;
-    if (tid == 0) { misc[50] = 0; misc[51] = 0; }
+    if (tid == 0) { misc[50] = 0; misc[51] = 0; if (app) misc[53] = 0; }
     if (sorted) {
         // ---- column statistics: min / max x1, max width
         T lo = (T)1e30, hi = (T)-1e30, mw = (T)0;
@@ -273,18 +332,34 @@ B2T_DEVNI bool build_csr(SeqView<T>& v, StepSmem<T>& sm, int n, int m, T thresh,
     B2T_SUB(4);
     // ---- stage 2: one thread per candidate pair
     const int nE = fits ? total : 0;
-    for (int e = tid; e < nE; e += nthr) {
-        // which storage holds entry e?  rows never straddle: a row is in shared memory iff it ends below esm
-        int* pc = sm.se_col; T* pw = sm.se_cost;
+    // which storage holds entry e?  rows never straddle: a row is in shared memory iff it ends below esm
+    auto locate = [&](int e, int*& pc, T*& pw) {
+        pc = sm.se_col; pw = sm.se_cost;
         int i = e < sm.esm ? sm.se_row[e] : -1;
         if (!(i >= 0 && i < n && sm.rstart[i] <= e && e < sm.rstart[i] + sm.rcnt[i] && sm.rstart[i] + sm.rcnt[i] <= sm.esm)) {
             pc = v.e_col; pw = v.e_cost; i = v.e_row[e];
         }
+        return i;
+    };
+    const T th_iou = app ? (T)app->theta_iou : (T)0;
+    for (int e = tid; e < nE; e += nthr) {
+        int* pc; T* pw;
+        const int i = locate(e, pc, pw);
         const int j = pc[e];
         const T cost = (T)1 - iou_plus1<T>(sm.rowbox + 4 * i, colbox + 4 * j);
-        if (cost < thresh) pw[e] = cost; else pc[e] = -1;
+        if (app && cost <= th_iou) { pw[e] = cost; v.e_app[atomicAdd(&misc[53], 1)] = pc == sm.se_col ? e : e | (int)0x80000000; }
+        else if (cost < thresh) pw[e] = cost;
+        else pc[e] = -1;
     }
     __syncthreads();
+    if (app) {
+        const int na = misc[53];
+        const int lowered = app_costs<T>(*app, v.feat, v.feat_dim, v.e_app, na, sm.se_col, sm.se_row, sm.se_cost, v.e_col, v.e_row,
+                                         v.e_cost, thresh);
+        if (lowered) atomicAdd(&misc[54], lowered);
+        if (tid == 0) misc[55] += na;
+        __syncthreads();
+    }
     B2T_SUB(5);
     return fits;
 }
@@ -313,10 +388,11 @@ template <class T> B2T_DEV LapCsr<T> step_csr(StepCtx<T>& c, int w2_base = 0, in
     return g;
 }
 
-template <class T> B2T_DEVNI void associate(StepCtx<T>& c, int n, int m, T thresh, int* err, long long* tsplit, int* dbg = nullptr) {
+template <class T> B2T_DEVNI void associate(StepCtx<T>& c, int n, int m, T thresh, int* err, long long* tsplit, int* dbg = nullptr,
+                                             const AppCtx* app = nullptr) {
     StepSmem<T>& sm = c.sm;
     long long dt = phase_clock();
-    const bool ok = build_csr<T>(c.v, sm, n, m, thresh, dbg, &dt);
+    const bool ok = build_csr<T>(c.v, sm, n, m, thresh, dbg, &dt, app);
     if (!ok && threadIdx.x == 0) *err |= ERR_EDGES;
     // The rows that did not fit the shared-memory edge mirror live in the global edge workspace.  rowbox / colbox are dead from
     // here to the next association (each one refills them): the first spilled rows are copied into that memory, so that the
@@ -392,11 +468,62 @@ B2T_DEVNI void apply_matches(StepCtx<T>& c, const int* rows, int n, const float*
     __syncthreads();
 }
 
+// Feature EMA of STrack.update with a high detection (basetrack.py:323-332) for the rows updated by apply_matches (rowdet[k] >= 0,
+// rowmode[k] == 0; re_activate leaves the feature alone), one warp per track, in float32 as NumPy 2 evaluates it:
+//   f^ = f / |f|,  s = 0.9 old + 0.1 f^,  s /= |s|.
+// The squared norms are summed in float64 and rounded once (NumPy's float32 dot sums in float32, in BLAS order).
+B2T_DEV float warp_norm_f32(const float4* x, int n4) {
+    double ss = 0.0;
+    for (int k = lane_id(); k < n4; k += 32) {
+        const float4 a = x[k];
+        ss += (double)a.x * a.x + (double)a.y * a.y + (double)a.z * a.z + (double)a.w * a.w;
+    }
+    for (int o = 16; o; o >>= 1) ss += shfl_xor(ss, o);
+    return sqrtf((float)ss);
+}
+B2T_DEVNI void ema_features(float* tfeat, int D, const int* rows, int n, const float* feats, const int* rowdet,
+                             const unsigned char* rowmode) {
+    const int D4 = D >> 2, lane = lane_id();
+    for (int k = warp_id(); k < n; k += num_warps()) {
+        const int d = rowdet[k];
+        if (d < 0 || rowmode[k] != 0) continue;
+        const float4* f = reinterpret_cast<const float4*>(feats + (size_t)d * D);
+        float4* s = reinterpret_cast<float4*>(tfeat + (size_t)rows[k] * D);
+        const float nf = warp_norm_f32(f, D4);
+        for (int q = lane; q < D4; q += 32) {
+            const float4 a = f[q], o = s[q];
+            float4 r;
+            r.x = 0.9f * o.x + 0.1f * (a.x / nf); r.y = 0.9f * o.y + 0.1f * (a.y / nf);
+            r.z = 0.9f * o.z + 0.1f * (a.z / nf); r.w = 0.9f * o.w + 0.1f * (a.w / nf);
+            s[q] = r;
+        }
+        const float ns = warp_norm_f32(s, D4);      // each lane re-reads only what it wrote
+        for (int q = lane; q < D4; q += 32) {
+            float4 r = s[q];
+            r.x = r.x / ns; r.y = r.y / ns; r.z = r.z / ns; r.w = r.w / ns;
+            s[q] = r;
+        }
+    }
+    __syncthreads();
+}
+
+// births: a new track keeps its detection's feature as the extractor returned it (STrack.__init__, basetrack.py:101-102)
+B2T_DEVNI void copy_features(float* tfeat, int D, const int* slots, const int* det_rows, int n, const float* feats) {
+    for (int k = warp_id(); k < n; k += num_warps()) {
+        const float4* src = reinterpret_cast<const float4*>(feats + (size_t)det_rows[k] * D);
+        float4* dst = reinterpret_cast<float4*>(tfeat + (size_t)slots[k] * D);
+        for (int q = lane_id(); q < (D >> 2); q += 32) dst[q] = src[q];
+    }
+    __syncthreads();
+}
+
 #define B2T_PHASE(idx) do { if (tid == 0) { const long long now_ = phase_clock(); stat[STAT_PHASE0 + (idx)] = (int)(now_ - tprev); tprev = now_; } } while (0)
 
-template <class T>
+// APP: the BoT-SORT-with-ReID instantiation (feat_dim > 0).  The IoU-only trackers run the APP = false one, which compiles to the
+// same code as without appearance support.
+template <class T, bool APP>
 B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq, const float* dets_all,
-                            const int* det_count, const double* warps, const int* id_base, double* out_all,
+                            const int* det_count, const float* feats_all, const double* warps, const int* id_base, double* out_all,
                             int out_rows, int* stat_all, unsigned char* smem_raw) {
     StepCtx<T> c(st, seq, prm);
     Arena arena(smem_raw);
@@ -411,8 +538,11 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
     int* stat = stat_all + (size_t)seq * STAT_WORDS;
     int* err = &sm.misc[48];
     long long tprev = phase_clock();
+    // detection features [dmax][feat_dim] of this sequence (BoT-SORT with ReID), null otherwise
+    const float* feats = APP && feats_all && !p.predict_only ? feats_all + (size_t)seq * st.dmax * st.feat_dim : nullptr;
 
     if (tid == 0) {
+        if (APP) { sm.misc[54] = 0; sm.misc[55] = 0; }
         for (int q = 0; q < 48; ++q) stat[STAT_PHASE0 + q] = 0;
         *err = v.ctrl[CTRL_ERR];
         if (id_base) v.ctrl[CTRL_NEXT_ID] = id_base[seq];
@@ -520,7 +650,8 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         __syncthreads();
         B2T_PHASE(3);
         long long tsplit = tprev;
-        associate<T>(c, npool, nhi, (T)p.t1, err, &tsplit, stat + STAT_SUB0);
+        const AppCtx app1 = {sm.pool, sm.hi, feats, p.theta_iou, p.theta_emb};
+        associate<T>(c, npool, nhi, (T)p.t1, err, &tsplit, stat + STAT_SUB0, feats ? &app1 : nullptr);
         if (tid == 0) { stat[STAT_PHASE0 + 4] = (int)(tsplit - tprev); tprev = tsplit;
                         stat[12] = sm.lap.scratch[45]; stat[13] = sm.lap.scratch[41]; stat[14] = sm.lap.scratch[43]; stat[15] = sm.misc[50]; }
         B2T_PHASE(5);
@@ -548,6 +679,7 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         }
         __syncthreads();
         apply_matches<T>(c, sm.pool, npool, dets, sm.ntr, sm.used);
+        if (feats) ema_features(v.feat, v.feat_dim, sm.pool, npool, feats, sm.ntr, sm.used);
         B2T_PHASE(6);
         if (sort) {
             // basetrack.py:429-433: unmatched Tracked rows become lost
@@ -591,7 +723,8 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         for (int k = tid; k < nud0; k += nthr)
             for (int q = 0; q < 4; ++q) sm.colbox[4 * k + q] = sm.detbox[4 * sm.udets0[k] + q];
         __syncthreads();
-        associate<T>(c, nunc, nud0, (T)p.t3, err, nullptr);
+        const AppCtx app3 = {sm.unconf, sm.udets0, feats, p.theta_iou, p.theta_emb};
+        associate<T>(c, nunc, nud0, (T)p.t3, err, nullptr, nullptr, feats ? &app3 : nullptr);
         for (int k = tid; k < nunc; k += nthr)
             if (x[k] < 0) { const int s = sm.unconf[k]; v.state[s] = ST_REMOVED; if (v.removed_at[s] == 0) v.removed_at[s] = f; }
         // births (q3: BoT-SORT walks every first-stage leftover, the others only third-stage leftovers)
@@ -605,6 +738,7 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         for (int k = tid; k < nunc; k += nthr) { const int xx = x[k]; sm.ntr[k] = xx < 0 ? -1 : sm.udets0[xx]; sm.used[k] = 0; }
         __syncthreads();
         apply_matches<T>(c, sm.unconf, nunc, dets, sm.ntr, sm.used);
+        if (feats) ema_features(v.feat, v.feat_dim, sm.unconf, nunc, feats, sm.ntr, sm.used);
 
         B2T_PHASE(8);
         // ---- P7: births (STrack.activate, basetrack.py:222-245)
@@ -638,6 +772,7 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
             }
         }
         __syncthreads();
+        if (feats) copy_features(v.feat, v.feat_dim, v.freelist, sm.births, nbirth, feats);
         for (int k = tid; k < nbirth; k += nthr) sm.births[k] = v.freelist[k];               // now slots
         if (tid == 0) v.ctrl[CTRL_NEXT_ID] = id0 + nbirth;
         // ---- P8: prune long-lost tracks (iterates the OLD lost list, bytetrack.py:180-183)
@@ -722,6 +857,7 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         stat[STAT_NOUT] = nout; stat[STAT_NEXT_ID] = v.ctrl[CTRL_NEXT_ID]; stat[STAT_NTRACKED] = nt2; stat[STAT_NLOST] = nl2;
         stat[STAT_ERR] = *err; stat[STAT_FRAME] = f; stat[STAT_NPOOL] = npool; stat[STAT_NBIRTH] = nbirth;
         stat[STAT_NHI] = nhi; stat[STAT_NLO] = nlo; stat[STAT_NEDGE] = sm.misc[50]; stat[STAT_NMATCH0] = nmatch0;
+        if (APP) { stat[STAT_NAPP] = sm.misc[55]; stat[STAT_NAPPLOW] = sm.misc[54]; }
     }
 }
 

@@ -30,7 +30,7 @@ static int check_launch(const char* what) {
     return B2T_OK;
 }
 extern "C" const char* b2t_last_error(void) { return g_err.c_str(); }
-extern "C" int b2t_version(void) { return 100; }
+extern "C" int b2t_version(void) { return 101; }
 extern "C" long long b2t_launch_count(void) { return g_launches; }
 
 // ------------------------------------------------------------------------------------------ Kalman kernels
@@ -221,12 +221,12 @@ __global__ void lap_solve_kernel(int n, int m, T thresh, const int* e_col, const
 }
 
 // ------------------------------------------------------------------------------------------ fused step
-template <class T>
+template <class T, bool APP>
 __global__ void __launch_bounds__(512, 1)
-track_step_kernel(TrackState st, StepParams prm, const float* dets, const int* det_count, const double* warps,
+track_step_kernel(TrackState st, StepParams prm, const float* dets, const int* det_count, const float* feats, const double* warps,
                   const int* id_base, double* out, int out_rows, int* stat) {
     B2T_DYN_SMEM(smem_raw);
-    track_step_cta<T>(st, prm, (int)blockIdx.x, dets, det_count, warps, id_base, out, out_rows, stat, smem_raw);
+    track_step_cta<T, APP>(st, prm, (int)blockIdx.x, dets, det_count, feats, warps, id_base, out, out_rows, stat, smem_raw);
 }
 
 __global__ void track_reset_kernel(TrackState st) {
@@ -440,6 +440,10 @@ static void layout(const b2t_tracker_config& c, unsigned char* base, b2t_tracker
     TAKE(d_idbase, int, S); TAKE(d_out, double, S * cap * OUT_COLS); TAKE(d_stat, int, S * STAT_WORDS);
     TAKE(d_slot, double, 72);
     TAKE(d_list, double, cap * LIST_COLS + 1);
+    if (c.feat_dim > 0) {
+        TAKE(st.feat, float, S * cap * (size_t)c.feat_dim);
+        TAKE(st.e_app, int, S * (size_t)c.ecap);
+    }
 #undef TAKE
     *total = align_up(L.off, 256);
 }
@@ -450,6 +454,14 @@ static int check_cfg(const b2t_tracker_config* c) {
         return fail(B2T_EINVAL, "b2t_tracker: bad kind / fmt / dtype");
     if (c->n_seq < 1 || c->cap < 64 || c->dmax < 1 || c->dmax > 1024 || c->cap > 4096 || c->ecap < 1)
         return fail(B2T_EINVAL, "b2t_tracker: bad n_seq / cap (64..4096) / dmax (1..1024) / ecap");
+    if (c->feat_dim != 0) {
+        if (c->kind != B2T_BOTSORT) return fail(B2T_EINVAL, "b2t_tracker: feat_dim > 0 (appearance features) is only built for B2T_BOTSORT");
+        if (c->feat_dim < 0 || c->feat_dim % 32 != 0 || c->feat_dim > 2048)
+            return fail(B2T_EINVAL, "b2t_tracker: feat_dim must be 0 or a multiple of 32 up to 2048");
+        // theta_iou < 1 keeps every pair with an appearance cost among the overlapping ones (the sparse candidate set)
+        if (!(c->theta_iou < 1.0) || c->theta_emb != c->theta_emb)
+            return fail(B2T_EINVAL, "b2t_tracker: theta_iou must be < 1 and theta_emb a number");
+    }
     const size_t smem = c->dtype == B2T_F64 ? StepSmem<double>::bytes(c->cap, c->dmax, 0) : StepSmem<float>::bytes(c->cap, c->dmax, 0);
     if (smem > 227 * 1024) return fail(B2T_ECAPACITY, "b2t_tracker: cap / dmax need more than 227 KB of shared memory per CTA");
     return B2T_OK;
@@ -476,7 +488,7 @@ extern "C" int b2t_tracker_create(const b2t_tracker_config* cfg, void* state_mem
     t->cfg = *cfg;
     size_t total;
     layout(*cfg, (unsigned char*)state_mem, t, &total);
-    t->st.n_seq = cfg->n_seq; t->st.cap = cfg->cap; t->st.dmax = cfg->dmax; t->st.ecap = cfg->ecap;
+    t->st.n_seq = cfg->n_seq; t->st.cap = cfg->cap; t->st.dmax = cfg->dmax; t->st.ecap = cfg->ecap; t->st.feat_dim = cfg->feat_dim;
     t->st.esm = cfg->dtype == B2T_F64 ? StepSmem<double>::fit_esm(cfg->cap, cfg->dmax, cfg->ecap, 227 * 1024)
                                       : StepSmem<float>::fit_esm(cfg->cap, cfg->dmax, cfg->ecap, 227 * 1024);
     t->out_rows_cap = cfg->cap;
@@ -492,9 +504,13 @@ extern "C" int b2t_tracker_create(const b2t_tracker_config* cfg, void* state_mem
     p.t_dup = 0.15;                                                                           // basetrack.py:565
     p.max_time_lost = (int)(cfg->frame_rate / 30.0 * cfg->track_buffer);                      // basetrack.py:355-356
     p.use_gmc = cfg->use_gmc; p.predict_only = 0;
+    p.theta_iou = cfg->theta_iou; p.theta_emb = cfg->theta_emb;                               // botsort.py:289
     t->smem = cfg->dtype == B2T_F64 ? StepSmem<double>::bytes(cfg->cap, cfg->dmax, t->st.esm) : StepSmem<float>::bytes(cfg->cap, cfg->dmax, t->st.esm);
-    if (cfg->dtype == B2T_F64) { auto k = track_step_kernel<double>; if (B2T_SET_SMEM(k, t->smem) != 0) { delete t; return fail(B2T_ECUDA, "cannot raise dynamic shared memory"); } }
-    else { auto k = track_step_kernel<float>; if (B2T_SET_SMEM(k, t->smem) != 0) { delete t; return fail(B2T_ECUDA, "cannot raise dynamic shared memory"); } }
+    const bool app = cfg->feat_dim > 0;
+    int rs;
+    if (cfg->dtype == B2T_F64) rs = app ? B2T_SET_SMEM((track_step_kernel<double, true>), t->smem) : B2T_SET_SMEM((track_step_kernel<double, false>), t->smem);
+    else rs = app ? B2T_SET_SMEM((track_step_kernel<float, true>), t->smem) : B2T_SET_SMEM((track_step_kernel<float, false>), t->smem);
+    if (rs != 0) { delete t; return fail(B2T_ECUDA, "cannot raise dynamic shared memory"); }
     *out = t;
     return b2t_tracker_reset(t, stream);
 }
@@ -503,21 +519,55 @@ extern "C" void b2t_tracker_destroy(b2t_tracker* t) { delete t; }
 extern "C" int b2t_tracker_out_cols(void) { return OUT_COLS; }
 extern "C" int b2t_tracker_stat_words(void) { return STAT_WORDS; }
 
-extern "C" int b2t_tracker_step(b2t_tracker* t, const float* dets, const int* det_count, const double* warps,
-                                const int* id_base, double* out, int out_rows, int* stat, int predict_only, void* stream) {
-    if (!t || !out || !stat || out_rows < 1) return fail(B2T_EINVAL, "b2t_tracker_step: bad arguments");
+static int step_launch(b2t_tracker* t, const float* dets, const int* det_count, const float* feats, const double* warps,
+                       const int* id_base, double* out, int out_rows, int* stat, int predict_only, void* stream) {
+    if (!out || !stat || out_rows < 1) return fail(B2T_EINVAL, "b2t_tracker_step: bad arguments");
     if (!predict_only && (!dets || !det_count)) return fail(B2T_EINVAL, "b2t_tracker_step: dets / det_count are NULL");
     StepParams p = t->prm;
     p.predict_only = predict_only ? 1 : 0;
     cudaStream_t s = (cudaStream_t)stream;
+    const bool app = t->cfg.feat_dim > 0;
     if (t->cfg.dtype == B2T_F64) {
-        auto k = track_step_kernel<double>;
-        B2T_LAUNCH(k, t->cfg.n_seq, 512, t->smem, s, t->st, p, dets, det_count, warps, id_base, out, out_rows, stat);
+        auto k = app ? track_step_kernel<double, true> : track_step_kernel<double, false>;
+        B2T_LAUNCH(k, t->cfg.n_seq, 512, t->smem, s, t->st, p, dets, det_count, feats, warps, id_base, out, out_rows, stat);
     } else {
-        auto k = track_step_kernel<float>;
-        B2T_LAUNCH(k, t->cfg.n_seq, 512, t->smem, s, t->st, p, dets, det_count, warps, id_base, out, out_rows, stat);
+        auto k = app ? track_step_kernel<float, true> : track_step_kernel<float, false>;
+        B2T_LAUNCH(k, t->cfg.n_seq, 512, t->smem, s, t->st, p, dets, det_count, feats, warps, id_base, out, out_rows, stat);
     }
     return check_launch("track_step");
+}
+
+extern "C" int b2t_tracker_step(b2t_tracker* t, const float* dets, const int* det_count, const double* warps,
+                                const int* id_base, double* out, int out_rows, int* stat, int predict_only, void* stream) {
+    if (!t) return fail(B2T_EINVAL, "b2t_tracker_step: bad arguments");
+    if (t->cfg.feat_dim > 0) return fail(B2T_EINVAL, "b2t_tracker_step: this tracker carries appearance features, use b2t_tracker_step_feat");
+    return step_launch(t, dets, det_count, nullptr, warps, id_base, out, out_rows, stat, predict_only, stream);
+}
+
+extern "C" int b2t_tracker_step_feat(b2t_tracker* t, const float* dets, const int* det_count, const float* feats, const double* warps,
+                                     const int* id_base, double* out, int out_rows, int* stat, int predict_only, void* stream) {
+    if (!t) return fail(B2T_EINVAL, "b2t_tracker_step_feat: bad arguments");
+    if (t->cfg.feat_dim == 0) return fail(B2T_EINVAL, "b2t_tracker_step_feat: this tracker was created with feat_dim = 0, use b2t_tracker_step");
+    if (!predict_only && !feats) return fail(B2T_EINVAL, "b2t_tracker_step_feat: feats is NULL");
+    if (((size_t)feats & 15) != 0) return fail(B2T_EINVAL, "b2t_tracker_step_feat: feats must be 16-B aligned");
+    return step_launch(t, dets, det_count, feats, warps, id_base, out, out_rows, stat, predict_only, stream);
+}
+
+extern "C" int b2t_tracker_set_thetas(b2t_tracker* t, double theta_iou, double theta_emb) {
+    if (!t || t->cfg.feat_dim == 0) return fail(B2T_EINVAL, "b2t_tracker_set_thetas: no tracker with appearance features");
+    if (!(theta_iou < 1.0) || theta_emb != theta_emb) return fail(B2T_EINVAL, "b2t_tracker_set_thetas: theta_iou must be < 1 and theta_emb a number");
+    t->prm.theta_iou = theta_iou; t->prm.theta_emb = theta_emb;
+    return B2T_OK;
+}
+
+extern "C" int b2t_tracker_read_feature(b2t_tracker* t, int seq, int slot, float* host, void* stream) {
+    if (!t || t->cfg.feat_dim == 0 || seq < 0 || seq >= t->cfg.n_seq || slot < 0 || slot >= t->cfg.cap || !host)
+        return fail(B2T_EINVAL, "b2t_tracker_read_feature: bad arguments (or a tracker without appearance features)");
+    cudaStream_t s = (cudaStream_t)stream;
+    const size_t D = (size_t)t->cfg.feat_dim;
+    cudaMemcpyAsync(host, t->st.feat + ((size_t)seq * t->cfg.cap + slot) * D, D * sizeof(float), cudaMemcpyDeviceToHost, s);
+    if (cudaStreamSynchronize(s) != cudaSuccess) return fail(B2T_ECUDA, "b2t_tracker_read_feature: sync failed");
+    return B2T_OK;
 }
 
 extern "C" int b2t_tracker_step_host(b2t_tracker* t, const float* dets_host, const int* det_count_host,

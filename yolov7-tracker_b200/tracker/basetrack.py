@@ -258,8 +258,8 @@ class _TrackView(STrack):
             self.tracklet_len, self.start_frame, self.frame_id = int(extra[2]), int(extra[3]), int(extra[4])
             self.time_since_update = frame_id - self.frame_id
         self.kalman_format = kalman_format
-        self.features = []
-        self.has_feature = False
+        self._features = None
+        self.has_feature = engine.feat_dim > 0
         self._mean = self._cov = None
 
     @property
@@ -270,12 +270,31 @@ class _TrackView(STrack):
     def _tlwh(self):
         return self._row[1:5].astype(np.float32)
 
+    def _check_frame(self, what):
+        if self._engine.np_stat[self._seq, L.STAT_FRAME] != self._view_frame:
+            raise RuntimeError("track %d: %s were not read at frame %d and the tracker has moved on (frame %d): read them "
+                               "in the frame the track was returned" % (self.track_id, what, self._view_frame, int(self._engine.np_stat[self._seq, L.STAT_FRAME])))
+
     def _fetch(self):
         if self._mean is None:
-            if self._engine.np_stat[self._seq, L.STAT_FRAME] != self._view_frame:
-                raise RuntimeError("track %d: mean / cov were not read at frame %d and the tracker has moved on (frame %d): read them "
-                                   "in the frame the track was returned" % (self.track_id, self._view_frame, int(self._engine.np_stat[self._seq, L.STAT_FRAME])))
+            self._check_frame("mean / cov")
             self._mean, self._cov = self._engine.read_slot(self._seq, self._slot)
+
+    @property
+    def features(self):
+        """[smoothed appearance feature] (BoT-SORT with ReID, read from the device on first access, in the frame the view was made)
+        or [] without appearance features."""
+        if self._features is None:
+            if not self.has_feature:
+                self._features = []
+            else:
+                self._check_frame("features")
+                self._features = [self._engine.read_feature(self._seq, self._slot)]
+        return self._features
+
+    @features.setter
+    def features(self, v):
+        self._features = v
 
     @property
     def mean(self):
@@ -358,7 +377,7 @@ class BaseTracker(object):
         fmt = self.opts.kalman_format
         return [_TrackView(self._engine, 0, r, fmt, self.frame_id, extra=r[8:13]) for r in rows]
 
-    def _get_engine(self):
+    def _get_engine(self, feat_dim=0):
         if self._engine is None:
             from b200track.engine import TrackEngine
             if self.opts.kalman_format == 'naive':
@@ -366,7 +385,10 @@ class BaseTracker(object):
             self._engine = TrackEngine(kind=self._kind, n_seq=1, kalman_format=self.opts.kalman_format,
                                        conf_thresh=self.opts.conf_thresh, iou_thresh=getattr(self.opts, 'iou_thresh', 0.5),
                                        track_buffer=self.opts.track_buffer, frame_rate=self._frame_rate,
-                                       use_gmc=getattr(self, 'use_GMC', False), **self._engine_kw)
+                                       use_gmc=getattr(self, 'use_GMC', False), feat_dim=feat_dim, **self._engine_kw)
+        if self._engine.feat_dim != feat_dim:
+            raise RuntimeError("the tracker started with %s appearance features and now runs with %s: set use_apperance_model before "
+                               "the first update" % (self._engine.feat_dim or "no", feat_dim or "none"))
         return self._engine
 
     @staticmethod
@@ -380,10 +402,14 @@ class BaseTracker(object):
 
     def _step(self, det_results, ori_img, predict_only=False):
         if getattr(self, 'use_apperance_model', False):
-            # reference bytetrack.py:78-86 / botsort.py:352-392: appearance costs fused into the association.  The extractor
-            # (reid_models.deepsort_reid.Extractor) and the cosine GEMM (matching.embedding_distance) run on the GPU, the fusion
-            # inside the fused per-frame kernel is not built -- and the reference ships it switched off.
-            raise NotImplementedError("use_apperance_model=True: the appearance cost is not fused into the GPU tracker step")
+            if self._kind != 'botsort':
+                # ByteTrack's appearance mode (reference bytetrack.py:109-113) mixes gamma * IoU + (1 - gamma) * appearance into a DENSE
+                # cost -- every track / detection pair becomes a candidate -- which the fused step's sparse assignment over
+                # overlapping pairs cannot hold.  BoT-SORT's gated min(IoU, appearance) keeps the overlap structure and is built.
+                raise NotImplementedError("use_apperance_model=True is built for BoTSORT only: %s's appearance cost is dense "
+                                          "(gamma * IoU + (1 - gamma) * appearance over every pair) and needs another assignment path"
+                                          % type(self).__name__)
+            return self._finish_step(self._step_appearance(det_results, ori_img, predict_only))
         eng = self._get_engine()
         self.frame_id += 1
         warp = None
@@ -399,6 +425,11 @@ class BaseTracker(object):
                 warp = self._warp(dets, ori_img)
             rows = eng.step_host(warps=None if warp is None else np.asarray(warp, dtype=np.float64).reshape(1, 6),
                                  id_base=[BaseTrack._count], predict_only=predict_only)[0]
+        return self._finish_step(rows)
+
+    def _finish_step(self, rows):
+        """Track views of the step's output rows; the id counter and the removed-list bookkeeping follow the engine."""
+        eng = self._engine
         BaseTrack._count = int(eng.np_stat[0, L.STAT_NEXT_ID])
         rows = rows.copy()
         fmt = self.opts.kalman_format

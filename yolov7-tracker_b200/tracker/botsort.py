@@ -117,3 +117,53 @@ class BoTSORT(BaseTracker):
             return None
         det_high = dets[dets[:, 4] >= np.float32(self.det_thresh)]            # reference :380 hands over the high-score detections
         return self.gmc.apply(raw_frame=ori_img, detections=det_high)
+
+    def get_feature(self, tlbrs, ori_img):
+        """Reference :291-311: the features of the crops ``ori_img[int(y1):int(y2), int(x1):int(x2)]``, one extractor call.  The
+        drop-in ``Extractor`` (or a ``ReidExtractor``) crops and runs on the device and returns a CUDA tensor; any other
+        ``reid_model(list_of_crops)`` callable gets the crops as the reference cuts them."""
+        if len(tlbrs) == 0:
+            return np.array([])
+        from reid_models.deepsort_reid import Extractor
+        from b200track.reid import ReidExtractor
+        net = self.reid_model.net if isinstance(self.reid_model, Extractor) else self.reid_model
+        if isinstance(net, ReidExtractor):
+            return net.features_from_frame(ori_img, tlbrs)
+        img = ori_img.cpu().numpy() if isinstance(ori_img, torch.Tensor) else ori_img
+        crops = []
+        for tlbr in tlbrs:
+            x1, y1, x2, y2 = list(map(int, tlbr))
+            crops.append(img[y1:y2, x1:x2])
+        return self.reid_model(crops)
+
+    def _step_appearance(self, det_results, ori_img, predict_only):
+        """BoTSORT.update with use_apperance_model (reference :313-493): the features of exactly the reference's det_high rows
+        (score >= det_thresh in float32, row order) come from ONE extractor call -- the extractor's batch-statistics BatchNorm makes a
+        feature depend on the crops that share the call -- and go to the fused step row-aligned with the detections."""
+        if self.reid_model is None:                                            # reference :278 builds it in the constructor
+            from reid_models.deepsort_reid import Extractor
+            self.reid_model = Extractor(self.opts.reid_model_path, use_cuda=True)
+        self.frame_id += 1
+        if predict_only:
+            eng = self._get_engine(self._engine.feat_dim if self._engine is not None else 512)
+            eng.set_thetas(self.theta_iou, self.theta_emb)
+            return eng.step_cuda_dets([torch.zeros((0, 6), device=eng.device)], id_base=[BaseTrack._count], feats_list=None,
+                                      predict_only=True)[0].copy()
+        dets = self._to_numpy(det_results)
+        hi = np.nonzero(dets[:, 4] >= np.float32(self.det_thresh))[0]
+        feats = self.get_feature(dets[hi, :4], ori_img) if len(hi) else None
+        if feats is not None:
+            feats = feats if isinstance(feats, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(feats, dtype=np.float32))
+            if feats.dim() != 2 or feats.shape[0] != len(hi):
+                raise ValueError("reid_model returned features of shape %s for %d crops" % (tuple(feats.shape), len(hi)))
+        dim = int(feats.shape[1]) if feats is not None else (self._engine.feat_dim if self._engine is not None else 512)
+        if dim % 32 or dim > 2048:
+            raise ValueError("appearance features of length %d: the fused step takes a multiple of 32 up to 2048" % dim)
+        eng = self._get_engine(dim)
+        eng.set_thetas(self.theta_iou, self.theta_emb)                         # plain attributes, read every frame as the reference does
+        rows = torch.zeros((len(dets), dim), dtype=torch.float32, device=eng.device)
+        if feats is not None:
+            rows[torch.from_numpy(hi).to(eng.device)] = feats.to(eng.device, torch.float32)
+        warp = self._warp(dets, ori_img)
+        return eng.step_cuda_dets([torch.from_numpy(dets).to(eng.device)], feats_list=[rows], id_base=[BaseTrack._count],
+                                  warps=None if warp is None else np.asarray(warp, dtype=np.float64).reshape(1, 6))[0].copy()
