@@ -321,9 +321,12 @@ int b2t_maxpool2x2s2(const void* in, void* out, int n, int h, int w, int c, int 
 int b2t_add_relu(const void* a, const void* b, void* out, long long n_elems, int act_dtype, void* stream);
 /* nn.BatchNorm2d with BATCH statistics -- the reference's extractor is never switched to eval() (deepsort_reid.py:112-121, :148-153), so
  * every call normalises with the mean and biased variance of that call's crops: y = (x - mean) / sqrt(var + eps) * gamma + beta
- * (+ ReLU) over x [n_pix][c]; sums_ws: 1024 doubles of scratch.  In place (y == x) is allowed. */
+ * (+ ReLU) over x [n_pix][c], 8 <= c <= 512, c % 8 == 0, 256 % (c / 8) == 0.  Statistics and normalisation in fp64, summed in a fixed
+ * order: the same input gives the same bits on every call.  ws: device scratch of at least b2t_batchnorm_workspace_bytes(n_pix, c)
+ * bytes (nothing carries over between calls).  In place (y == x) is allowed. */
+size_t b2t_batchnorm_workspace_bytes(long long n_pix, int c);      /* 0 for arguments b2t_batchnorm_batch_stats refuses */
 int b2t_batchnorm_batch_stats(const void* x, void* y, long long n_pix, int c, const float* gamma, const float* beta, float eps, int relu,
-                              double* sums_ws, int act_dtype, void* stream);
+                              double* ws, int act_dtype, void* stream);
 /* nn.AvgPool2d over the whole hw-position map (:83) + division by the L2 norm (:103-104): in [n][hw][512] -> out [n][512] fp32 */
 int b2t_avgpool_l2norm(const void* in, float* out, int n, int hw, int c, int act_dtype, void* stream);
 

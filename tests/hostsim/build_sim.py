@@ -1,4 +1,4 @@
-"""Builds tests/hostsim/libb2t_hostsim.so: the tracker kernels compiled by g++ against the fiber
+"""Builds tests/hostsim/libb2t_hostsim.so: the tracker, NMS, pre-processing, camera-motion and ReID glue kernels compiled by g++ against the fiber
 simulator (cuda_sim.h).  TEST INFRASTRUCTURE ONLY -- see cuda_sim.h.  The product never loads it."""
 import hashlib
 import os
@@ -27,6 +27,7 @@ def build(force=False):
     # -ffp-contract=off: no FMA contraction, like the nvcc build's --fmad=false
     cmd = ["g++", "-O2", "-g", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-DB2T_HOSTSIM",
            "-I", HERE, "-I", CSRC, "-x", "c++", os.path.join(CSRC, "b2t_tracker.cu"), "-x", "c++", os.path.join(CSRC, "b2t_nms.cu"), "-x", "c++", os.path.join(CSRC, "b2t_preproc.cu"), "-x", "c++", os.path.join(CSRC, "b2t_gmc.cu"),
+           "-x", "c++", os.path.join(CSRC, "b2t_reid.cu"),
            "-x", "c++", os.path.join(HERE, "cuda_sim.cpp"), "-o", LIB]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:

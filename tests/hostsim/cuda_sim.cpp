@@ -92,3 +92,17 @@ void run_block(int nthreads) {
     sim_switch(&g.sched_sp, g.fibers[0].sp);
 }
 }  // namespace sim
+
+// the 16-bit conversions of cuda_sim.h, exported for tests/test_hostsim_reid.py (checked against NumPy / torch there)
+extern "C" void b2t_sim_to16(const double* in, unsigned short* out, long long n, int bf16) {
+    for (long long i = 0; i < n; ++i) out[i] = bf16 ? __double2bfloat16(in[i]).x : __double2half(in[i]).x;
+}
+extern "C" void b2t_sim_f32_to16(const float* in, unsigned short* out, long long n, int bf16) {
+    for (long long i = 0; i < n; ++i) out[i] = bf16 ? __float2bfloat16_rn(in[i]).x : __float2half_rn(in[i]).x;
+}
+extern "C" void b2t_sim_from16(const unsigned short* in, float* out, long long n, int bf16) {
+    for (long long i = 0; i < n; ++i) {
+        if (bf16) { __nv_bfloat16 h; h.x = in[i]; out[i] = __bfloat162float(h); }
+        else { __half h; h.x = in[i]; out[i] = __half2float(h); }
+    }
+}

@@ -9,7 +9,8 @@
 //
 // Supported: threadIdx/blockIdx/blockDim/gridDim (.x only), static + dynamic __shared__,
 // __syncthreads, __syncwarp, full-mask __shfl*_sync / __ballot_sync / __any_sync / __all_sync /
-// __match_any_sync, integer + fp atomics, and a handful of cudaMemcpy-style host calls.
+// __match_any_sync, integer + fp atomics (fp64 included), software __half / __nv_bfloat16 conversions, and a handful of
+// cudaMemcpy-style host calls.
 #pragma once
 #include <cstdint>
 #include <cstdio>
@@ -202,10 +203,51 @@ inline int __float2int_rn(float v) { return (int)lrintf(v); }      // round to n
 inline int min(int a, int b) { return a < b ? a : b; }
 inline int max(int a, int b) { return a > b ? a : b; }
 struct float4 { float x, y, z, w; };
+struct uint2 { unsigned x, y; };
 struct uint4 { unsigned x, y, z, w; };
 inline float4 make_float4(float x, float y, float z, float w) { float4 r; r.x = x; r.y = y; r.z = z; r.w = w; return r; }
 inline float __int_as_float(int v) { return sim::from_bits<float>((uint64_t)(uint32_t)v); }
 inline int __float_as_int(float v) { return (int)(uint32_t)sim::to_bits(v); }
+
+// ---- 16-bit floating point (cuda_fp16.h / cuda_bf16.h subset) in software: IEEE binary16 and bfloat16 bit patterns, conversions
+// rounded to nearest even straight from the (exact) float / double value, subnormals and overflow to infinity included.
+struct __half { unsigned short x; };
+struct __nv_bfloat16 { unsigned short x; };
+namespace sim {
+// round |v| to a binary format with `mant` stored significand bits and `expb` exponent bits -> bit pattern (sign included)
+inline unsigned short round16(double v, int mant, int expb) {
+    const unsigned sign = std::signbit(v) ? 1u << (mant + expb) : 0u;
+    const unsigned inf = ((1u << expb) - 1u) << mant;
+    if (std::isnan(v)) return (unsigned short)(sign | inf | (1u << (mant - 1)));
+    const double a = std::fabs(v);
+    if (std::isinf(a)) return (unsigned short)(sign | inf);
+    if (a == 0.0) return (unsigned short)sign;
+    const int bias = (1 << (expb - 1)) - 1, emin = 1 - bias;
+    int e;
+    std::frexp(a, &e);
+    int E = e - 1;                                          // a in [2^E, 2^(E+1))
+    if (E < emin) E = emin;                                 // subnormal range: fixed quantum 2^(emin - mant)
+    const double r = std::nearbyint(std::ldexp(a, mant - E)); // significand with `mant` fraction bits, rounded to nearest even
+    // ((E + bias - 1) << mant) + r: a subnormal when E == emin and r < 2^mant, and a carry out of the significand bumps the exponent
+    const double bits = std::ldexp((double)(E + bias - 1), mant) + r;
+    if (bits >= (double)inf) return (unsigned short)(sign | inf);
+    return (unsigned short)(sign | (unsigned)bits);
+}
+inline double widen16(unsigned short b, int mant, int expb) {
+    const int bias = (1 << (expb - 1)) - 1;
+    const unsigned m = b & ((1u << mant) - 1u), ex = (b >> mant) & ((1u << expb) - 1u);
+    const double sgn = (b >> (mant + expb)) & 1u ? -1.0 : 1.0;
+    if (ex == (1u << expb) - 1u) return m ? (double)NAN : sgn * (double)INFINITY;
+    if (ex == 0) return sgn * std::ldexp((double)m, 1 - bias - mant);
+    return sgn * std::ldexp((double)(m | (1u << mant)), (int)ex - bias - mant);
+}
+}  // namespace sim
+inline __half __double2half(double v) { __half h; h.x = sim::round16(v, 10, 5); return h; }
+inline __half __float2half_rn(float v) { return __double2half((double)v); }
+inline float __half2float(__half h) { return (float)sim::widen16(h.x, 10, 5); }
+inline __nv_bfloat16 __double2bfloat16(double v) { __nv_bfloat16 h; h.x = sim::round16(v, 7, 8); return h; }
+inline __nv_bfloat16 __float2bfloat16_rn(float v) { return __double2bfloat16((double)v); }
+inline float __bfloat162float(__nv_bfloat16 h) { return (float)sim::widen16(h.x, 7, 8); }
 
 // ---- host runtime shims (device memory == host memory) ----
 inline cudaError_t cudaMalloc(void** p, size_t n) { *p = malloc(n ? n : 1); return *p ? 0 : 2; }

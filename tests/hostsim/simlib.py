@@ -19,7 +19,7 @@ _sim = None
 def sim():
     global _sim
     if _sim is None:
-        _sim = L.declare(C.CDLL(build_sim.build()), names=L.TRACKER_SYMBOLS + L.NMS_SYMBOLS)   # the simulator builds the tracker and NMS TUs
+        _sim = L.declare(C.CDLL(build_sim.build()), names=L.TRACKER_SYMBOLS + L.NMS_SYMBOLS + L.REID_SYMBOLS)   # the TUs build_sim compiles
     return _sim
 
 

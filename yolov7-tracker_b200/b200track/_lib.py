@@ -101,6 +101,7 @@ SIGNATURES = {
     "b2t_maxpool2x2s2": (_I, [_P, _P, _I, _I, _I, _I, _I, _P]),
     "b2t_image_nhwc16": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "b2t_add_relu": (_I, [_P, _P, _P, C.c_longlong, _I, _P]),
+    "b2t_batchnorm_workspace_bytes": (_SZ, [C.c_longlong, _I]),
     "b2t_batchnorm_batch_stats": (_I, [_P, _P, C.c_longlong, _I, _P, _P, C.c_float, _I, _P, _I, _P]),
     "b2t_avgpool_l2norm": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "b2t_detect_nms": (_I, [_P, _I, _I, _I, C.c_float, C.c_float, _I, _I, _I, _I, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,
@@ -117,6 +118,10 @@ class HeadLevel(C.Structure):
 # the NMS translation unit also compiles for the host simulator (tests/hostsim)
 NMS_SYMBOLS = ["b2t_detect_last_error", "b2t_nms_workspace_bytes", "b2t_nms", "b2t_detect_nms", "b2t_letterbox", "b2t_letterbox_reorg",
                "b2t_gmc_workspace_bytes", "b2t_gmc_reset", "b2t_gmc_estimate", "b2t_gmc_workspace_layout", "b2t_gmc_prepare", "b2t_gmc_estimate_prepared"]
+
+# the appearance branch's element-wise kernels (csrc/b2t_reid.cu) also compile for the host simulator
+REID_SYMBOLS = ["b2t_reid_crops", "b2t_maxpool3x3s2", "b2t_maxpool2x2s2", "b2t_add_relu", "b2t_batchnorm_workspace_bytes", "b2t_batchnorm_batch_stats",
+                "b2t_avgpool_l2norm"]
 
 # the association branch (csrc/b2t_tracker.cu); the rest are the detector's translation units
 TRACKER_SYMBOLS = [n for n in SIGNATURES if not n.startswith(("b2t_conv", "b2t_detect", "b2t_image", "b2t_upsample", "b2t_spp", "b2t_nms", "b2t_letterbox", "b2t_gmc_workspace", "b2t_gmc_reset", "b2t_gmc_estimate", "b2t_gmc_prepare",

@@ -86,7 +86,6 @@ class ReidExtractor:
             self.weights[name] = (pack_conv_weight(w.to(self.dev), cin_pad=cin_pad, dtype=dtype), b.to(self.dev).float().contiguous(), w.shape[0], w.shape[1] if cin_pad is None else 16, k, s)
             if bn_mode == "batch":
                 self.bn[name] = (item[4].to(self.dev).float().contiguous(), item[5].to(self.dev).float().contiguous())
-        self.sums = torch.zeros(1024, dtype=torch.float64, device=self.dev)
         self._nets = {}
 
     def _stream(self):
@@ -98,6 +97,8 @@ class ReidExtractor:
         buf = lambda h, w, c: torch.zeros((n, h, w, c), dtype=dt, device=dev)          # noqa: E731
         net = {"n": n, "valid": n, "x": buf(128, 64, 16), "c0": buf(128, 64, 64), "ops": []}
         ops = net["ops"]
+        bn_ws = [None]                         # BatchNorm scratch, sized below for the largest layer of this capacity
+        bn_bytes = [0]
 
         def check(rc):
             if rc != 0:
@@ -112,9 +113,10 @@ class ReidExtractor:
             if batch:
                 g, beta = self.bn[name]
                 ho, wo = h // s, w // s
+                bn_bytes[0] = max(bn_bytes[0], int(self.lib.b2t_batchnorm_workspace_bytes(n * ho * wo, cout)))     # grows with n_pix
                 # statistics over the VALID crops only (net["valid"]): the rows that pad the batch to its capacity must not count
                 ops.append(lambda y=y, g=g, beta=beta, c=cout, hw=ho * wo, relu=int(act == 2): check(self.lib.b2t_batchnorm_batch_stats(
-                    y.data_ptr(), y.data_ptr(), net["valid"] * hw, c, g.data_ptr(), beta.data_ptr(), EPS, relu, self.sums.data_ptr(), self.code, self._stream())))
+                    y.data_ptr(), y.data_ptr(), net["valid"] * hw, c, g.data_ptr(), beta.data_ptr(), EPS, relu, bn_ws[0].data_ptr(), self.code, self._stream())))
             return plan
         net["plans"] = [conv("conv0", net["x"], net["c0"], 128, 64, 2)]
         cur = buf(64, 32, 64)
@@ -136,6 +138,8 @@ class ReidExtractor:
                 ops.append(lambda a=skip, b=y2, o=out: check(self.lib.b2t_add_relu(a.data_ptr(), b.data_ptr(), o.data_ptr(), a.numel(), self.code, self._stream())))
                 net.setdefault("keep", []).extend([y1, y2, skip, out])
                 cur, h, w = out, ho, wo
+        if self.bn_mode == "batch":
+            bn_ws[0] = net["bn_ws"] = torch.zeros((bn_bytes[0] + 7) // 8, dtype=torch.float64, device=dev)
         net["feat"] = torch.zeros((n, 512), dtype=torch.float32, device=dev)
         last = cur
         ops.append(lambda a=last, o=net["feat"]: check(self.lib.b2t_avgpool_l2norm(a.data_ptr(), o.data_ptr(), n, h * w, 512, self.code, self._stream())))
@@ -180,6 +184,9 @@ class ReidExtractor:
         f = f.to(self.dev).contiguous()
         H, W = int(f.shape[0]), int(f.shape[1])
         t = np.asarray(tlbrs, dtype=np.float64).reshape(-1, 4).astype(np.int64)                 # list(map(int, tlbr)): truncation
+        if (t < 0).any():
+            # ori_img[int(y1):int(y2), int(x1):int(x2)] would wrap a negative index to the far side of the frame
+            raise L.B2TError("ReidExtractor: a box has a negative coordinate after int() (clip the boxes to the frame first)")
         x1, y1 = np.clip(t[:, 0], 0, W), np.clip(t[:, 1], 0, H)
         x2, y2 = np.clip(t[:, 2], 0, W), np.clip(t[:, 3], 0, H)
         if ((x2 - x1) < 1).any() or ((y2 - y1) < 1).any():

@@ -8,9 +8,11 @@
 //   avgpool_l2norm_kernel  nn.AvgPool2d((8, 4), 1) :83 + x.div(x.norm(p=2, dim=1)) :103-104 -> 512 floats per crop
 #include <string>          // before b2t_platform.cuh (the simulator's __noinline__ macro must not reach libstdc++)
 #include <math.h>
-#include <cuda_fp16.h>
-#include <cuda_bf16.h>
 #include "b2t_platform.cuh"
+#if !defined(B2T_HOSTSIM)
+#include <cuda_fp16.h>                // the host simulator brings its own __half / __nv_bfloat16 (tests/hostsim/cuda_sim.h)
+#include <cuda_bf16.h>
+#endif
 #include "../../include/b200track.h"
 
 namespace b2t { void set_detect_error(const char* m); }
@@ -139,35 +141,89 @@ __global__ void avgpool_l2norm_kernel(const unsigned short* __restrict__ in, flo
 }
 
 // ---- BatchNorm with BATCH statistics.  The reference never calls net.eval() (deepsort_reid.py:112-121, :148-153): its BatchNorm layers
-// normalise every call with the mean / biased variance of that call's crops.  Reproduced as two passes over the conv output:
-// per-channel sums (fp32 partials per block, fp64 atomics), then scale / shift (+ ReLU).  x: [n_pix][c] 16-bit, c <= 512, c % 8 == 0.
-__global__ void bn_stats_kernel(const unsigned short* __restrict__ x, long long n_pix, int c, double* __restrict__ sums, int f16) {
+// normalise every call with the mean / biased variance of that call's crops.  x: [n_pix][c] 16-bit, c <= 512, c % 8 == 0, 256 % (c / 8) == 0.
+// Three launches, all in a fixed summation order, so the result is bitwise reproducible from call to call:
+//   bn_stats_kernel     block b: fp64 sums of (x - K) and (x - K)^2 per channel over its pixels, K = the channel's value at pixel 0 (a shift
+//                       inside the data keeps the variance free of the E[x^2] - mean^2 cancellation); per-block partials -> ws
+//   bn_finalize_kernel  per channel: the partials of all blocks in block order -> mean and gamma / sqrt(var + eps) (fp64) -> ws[0 .. 2c)
+//   bn_apply_kernel     y = (x - mean) * scale + beta (+ ReLU) in fp64, rounded once to the 16-bit type
+// ws layout (doubles): [0, c) mean, [c, 2c) scale, then [block][2][c] partials.
+constexpr int kBnThreads = 256;
+constexpr int kBnMaxBlocks = 132 * 8;
+constexpr int kBnFinalWarps = 32;
+
+int bn_blocks(long long n_pix, int c) {
+    const long long ppb = kBnThreads / (c / 8);
+    const long long g = (n_pix + ppb * 16 - 1) / (ppb * 16);
+    return (int)(g < 1 ? 1 : (g > kBnMaxBlocks ? kBnMaxBlocks : g));
+}
+
+__device__ __forceinline__ unsigned short store16_d(double v, int f16) {
+    if (f16) { const __half h = __double2half(v); return *reinterpret_cast<const unsigned short*>(&h); }
+    const __nv_bfloat16 h = __double2bfloat16(v); return *reinterpret_cast<const unsigned short*>(&h);
+}
+
+__global__ void bn_stats_kernel(const unsigned short* __restrict__ x, long long n_pix, int c, double* __restrict__ ws, int f16) {
     // thread t handles the 8-channel vector (t % cv) of pixels t / cv, t / cv + stride ...
     const int cv = c / 8;
     const int vec = threadIdx.x % cv, lane_pix = threadIdx.x / cv, pix_per_block = blockDim.x / cv;
-    float s[8], q[8];
+    double shift[8], s[8], q[8];
+    {
+        const uint4 v = *reinterpret_cast<const uint4*>(x + vec * 8);
+        const unsigned short* e = reinterpret_cast<const unsigned short*>(&v);
 #pragma unroll
-    for (int k = 0; k < 8; ++k) { s[k] = 0.f; q[k] = 0.f; }
-    if (lane_pix < pix_per_block)
-        for (long long p = (long long)blockIdx.x * pix_per_block + lane_pix; p < n_pix; p += (long long)gridDim.x * pix_per_block) {
-            const uint4 v = *reinterpret_cast<const uint4*>(x + p * c + vec * 8);
-            const unsigned short* e = reinterpret_cast<const unsigned short*>(&v);
+        for (int k = 0; k < 8; ++k) { shift[k] = (double)load16(e + k, f16); s[k] = 0.0; q[k] = 0.0; }
+    }
+    for (long long p = (long long)blockIdx.x * pix_per_block + lane_pix; p < n_pix; p += (long long)gridDim.x * pix_per_block) {
+        const uint4 v = *reinterpret_cast<const uint4*>(x + p * c + vec * 8);
+        const unsigned short* e = reinterpret_cast<const unsigned short*>(&v);
 #pragma unroll
-            for (int k = 0; k < 8; ++k) { const float f = load16(e + k, f16); s[k] += f; q[k] += f * f; }
-        }
-    __shared__ float sh[2][512];
-    for (int i = threadIdx.x; i < 2 * 512; i += blockDim.x) (&sh[0][0])[i] = 0.f;
+        for (int k = 0; k < 8; ++k) { const double d = (double)load16(e + k, f16) - shift[k]; s[k] += d; q[k] += d * d; }
+    }
+    // fixed-order tree over the block's pixel lanes: lane l adds lane l + st for st = pix_per_block / 2 .. 1 (a power of two)
+    __shared__ double sh[16][kBnThreads];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) { sh[k][threadIdx.x] = s[k]; sh[8 + k][threadIdx.x] = q[k]; }
     __syncthreads();
-    if (lane_pix < pix_per_block)
+    for (int st = pix_per_block / 2; st >= 1; st >>= 1) {
+        if (lane_pix < st)
 #pragma unroll
-        for (int k = 0; k < 8; ++k) { atomicAdd(&sh[0][vec * 8 + k], s[k]); atomicAdd(&sh[1][vec * 8 + k], q[k]); }
-    __syncthreads();
-    for (int i = threadIdx.x; i < c; i += blockDim.x) { atomicAdd(&sums[i], (double)sh[0][i]); atomicAdd(&sums[512 + i], (double)sh[1][i]); }
+            for (int k = 0; k < 16; ++k) sh[k][threadIdx.x] += sh[k][threadIdx.x + st * cv];
+        __syncthreads();
+    }
+    if (lane_pix == 0) {
+        double* part = ws + 2 * c + (size_t)blockIdx.x * 2 * c;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) { part[vec * 8 + k] = sh[k][threadIdx.x]; part[c + vec * 8 + k] = sh[8 + k][threadIdx.x]; }
+    }
 }
 
-// y = (x - mean) / sqrt(var + eps) * gamma + beta, optional ReLU; also clears the sums for the next use
-__global__ void bn_apply_kernel(const unsigned short* __restrict__ x, unsigned short* __restrict__ y, long long n_vec, int c, long long n_pix,
-                                const double* __restrict__ sums, const float* __restrict__ gamma, const float* __restrict__ beta, float eps, int relu, int f16) {
+// block of kBnFinalWarps warps per 32 channels: lane = channel, warp w sums the partials of blocks w, w + 32, ... in order; then the
+// warps' totals in warp order
+__global__ void bn_finalize_kernel(const unsigned short* __restrict__ x, long long n_pix, int c, int blocks, const float* __restrict__ gamma,
+                                   float eps, double* __restrict__ ws, int f16) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, ch = blockIdx.x * 32 + lane;
+    double s = 0.0, q = 0.0;
+    if (ch < c)
+        for (int b = warp; b < blocks; b += kBnFinalWarps) {
+            const double* part = ws + 2 * c + (size_t)b * 2 * c;
+            s += part[ch]; q += part[c + ch];
+        }
+    __shared__ double red[2][kBnFinalWarps][32];
+    red[0][warp][lane] = s; red[1][warp][lane] = q;
+    __syncthreads();
+    if (warp == 0 && ch < c) {
+        s = 0.0; q = 0.0;
+        for (int w = 0; w < kBnFinalWarps; ++w) { s += red[0][w][lane]; q += red[1][w][lane]; }
+        const double m = s / (double)n_pix;                                        // mean of x - K
+        const double var = fmax(q / (double)n_pix - m * m, 0.0);                  // biased, like F.batch_norm in training mode
+        ws[ch] = (double)load16(x + ch, f16) + m;
+        ws[c + ch] = (double)gamma[ch] / sqrt(var + (double)eps);
+    }
+}
+
+__global__ void bn_apply_kernel(const unsigned short* __restrict__ x, unsigned short* __restrict__ y, long long n_vec, int c,
+                                const double* __restrict__ ws, const float* __restrict__ beta, int relu, int f16) {
     const int cv = c / 8;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n_vec; i += (long long)gridDim.x * blockDim.x) {
         const int vec = (int)(i % cv);
@@ -177,12 +233,9 @@ __global__ void bn_apply_kernel(const unsigned short* __restrict__ x, unsigned s
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
             const int ch = vec * 8 + k;
-            const double mean = sums[ch] / (double)n_pix;
-            const double var = fmax(sums[512 + ch] / (double)n_pix - mean * mean, 0.0);
-            const float sc = gamma[ch] * (float)(1.0 / sqrt(var + (double)eps));
-            float f = (load16(e + k, f16) - (float)mean) * sc + beta[ch];
-            if (relu) f = fmaxf(f, 0.f);
-            r.o[k] = store16(f, f16);
+            double f = ((double)load16(e + k, f16) - ws[ch]) * ws[c + ch] + (double)beta[ch];
+            if (relu) f = fmax(f, 0.0);
+            r.o[k] = store16_d(f, f16);
         }
         reinterpret_cast<uint4*>(y)[i] = r.q;
     }
@@ -190,51 +243,55 @@ __global__ void bn_apply_kernel(const unsigned short* __restrict__ x, unsigned s
 
 }  // namespace
 
+static int bn_args_ok(long long n_pix, int c) { return n_pix >= 1 && c >= 8 && c <= 512 && c % 8 == 0 && kBnThreads % (c / 8) == 0; }
+
+extern "C" size_t b2t_batchnorm_workspace_bytes(long long n_pix, int c) {
+    if (!bn_args_ok(n_pix, c)) return 0;
+    return ((size_t)2 * c + (size_t)bn_blocks(n_pix, c) * 2 * c) * sizeof(double);
+}
+
 extern "C" int b2t_batchnorm_batch_stats(const void* x, void* y, long long n_pix, int c, const float* gamma, const float* beta, float eps, int relu,
-                                         double* sums_ws, int act_dtype, void* stream) {
-    if (!x || !y || !gamma || !beta || !sums_ws || n_pix < 1 || c < 8 || c > 512 || c % 8) return rfail(B2T_EINVAL, "b2t_batchnorm_batch_stats: bad arguments (8 <= c <= 512, c % 8 == 0)");
+                                         double* ws, int act_dtype, void* stream) {
+    if (!x || !y || !gamma || !beta || !ws || n_pix < 1 || c < 8 || c > 512 || c % 8) return rfail(B2T_EINVAL, "b2t_batchnorm_batch_stats: bad arguments (8 <= c <= 512, c % 8 == 0)");
+    if (!bn_args_ok(n_pix, c)) return rfail(B2T_EINVAL, "b2t_batchnorm_batch_stats: c / 8 must divide 256");
     cudaStream_t s = (cudaStream_t)stream;
-    if (cudaMemsetAsync(sums_ws, 0, 1024 * sizeof(double), s) != cudaSuccess) return rfail(B2T_ECUDA, "b2t_batchnorm_batch_stats: memset failed");
-    const int cv = c / 8, threads = 256;                  // cv is a power of two <= 64 for the extractor's widths: 256 % cv == 0
-    if (threads % cv) return rfail(B2T_EINVAL, "b2t_batchnorm_batch_stats: c / 8 must divide 256");
-    const long long ppb = threads / cv;
-    long long g = (n_pix + ppb * 16 - 1) / (ppb * 16);
-    g = g < 1 ? 1 : (g > 132 * 8 ? 132 * 8 : g);
-    bn_stats_kernel<<<(int)g, threads, 0, s>>>((const unsigned short*)x, n_pix, c, sums_ws, act_dtype == B2T_ACT_F16);
-    bn_apply_kernel<<<grid_for(n_pix * cv, 256), 256, 0, s>>>((const unsigned short*)x, (unsigned short*)y, n_pix * cv, c, n_pix, sums_ws, gamma, beta, eps, relu,
-                                                           act_dtype == B2T_ACT_F16);
+    const int f16 = act_dtype == B2T_ACT_F16, g = bn_blocks(n_pix, c);
+    const unsigned short* xs = (const unsigned short*)x;
+    B2T_LAUNCH(bn_stats_kernel, g, kBnThreads, 0, s, xs, n_pix, c, ws, f16);
+    B2T_LAUNCH(bn_finalize_kernel, (c + 31) / 32, kBnFinalWarps * 32, 0, s, xs, n_pix, c, g, gamma, eps, ws, f16);
+    B2T_LAUNCH(bn_apply_kernel, grid_for(n_pix * (c / 8), 256), 256, 0, s, xs, (unsigned short*)y, n_pix * (c / 8), c, (const double*)ws, beta, relu, f16);
     return rcheck("batchnorm_batch_stats");
 }
 
 extern "C" int b2t_reid_crops(const unsigned char* pixels, const long long* crops, int n, void* out_nhwc16, int act_dtype, void* stream) {
     if (!pixels || !crops || !out_nhwc16 || n < 1 || (act_dtype != B2T_ACT_BF16 && act_dtype != B2T_ACT_F16)) return rfail(B2T_EINVAL, "b2t_reid_crops: bad arguments");
-    reid_crop_kernel<<<grid_for((long long)n * 128 * 64, 256), 256, 0, (cudaStream_t)stream>>>(pixels, crops, n, (unsigned short*)out_nhwc16, act_dtype == B2T_ACT_F16);
+    B2T_LAUNCH(reid_crop_kernel, grid_for((long long)n * 128 * 64, 256), 256, 0, (cudaStream_t)stream, pixels, crops, n, (unsigned short*)out_nhwc16, act_dtype == B2T_ACT_F16);
     return rcheck("reid_crops");
 }
 
 extern "C" int b2t_maxpool3x3s2(const void* in, void* out, int n, int h, int w, int c, int act_dtype, void* stream) {
     if (!in || !out || n < 1 || h < 1 || w < 1 || c < 8 || c % 8) return rfail(B2T_EINVAL, "b2t_maxpool3x3s2: bad arguments (channels must be a multiple of 8)");
-    maxpool_s2_kernel<<<grid_for((long long)n * ((h + 1) / 2) * ((w + 1) / 2) * (c / 8), 256), 256, 0, (cudaStream_t)stream>>>(
-        (const unsigned short*)in, (unsigned short*)out, n, h, w, c, act_dtype == B2T_ACT_F16, 3);
+    B2T_LAUNCH(maxpool_s2_kernel, grid_for((long long)n * ((h + 1) / 2) * ((w + 1) / 2) * (c / 8), 256), 256, 0, (cudaStream_t)stream,
+               (const unsigned short*)in, (unsigned short*)out, n, h, w, c, act_dtype == B2T_ACT_F16, 3);
     return rcheck("maxpool3x3s2");
 }
 
 extern "C" int b2t_maxpool2x2s2(const void* in, void* out, int n, int h, int w, int c, int act_dtype, void* stream) {
     if (!in || !out || n < 1 || h < 2 || w < 2 || (h & 1) || (w & 1) || c < 8 || c % 8) return rfail(B2T_EINVAL, "b2t_maxpool2x2s2: bad arguments (even sides, channels a multiple of 8)");
-    maxpool_s2_kernel<<<grid_for((long long)n * (h / 2) * (w / 2) * (c / 8), 256), 256, 0, (cudaStream_t)stream>>>(
-        (const unsigned short*)in, (unsigned short*)out, n, h, w, c, act_dtype == B2T_ACT_F16, 2);
+    B2T_LAUNCH(maxpool_s2_kernel, grid_for((long long)n * (h / 2) * (w / 2) * (c / 8), 256), 256, 0, (cudaStream_t)stream,
+               (const unsigned short*)in, (unsigned short*)out, n, h, w, c, act_dtype == B2T_ACT_F16, 2);
     return rcheck("maxpool2x2s2");
 }
 
 extern "C" int b2t_add_relu(const void* a, const void* b, void* out, long long n_elems, int act_dtype, void* stream) {
     if (!a || !b || !out || n_elems < 8 || n_elems % 8) return rfail(B2T_EINVAL, "b2t_add_relu: element count must be a multiple of 8");
-    add_relu_kernel<<<grid_for(n_elems / 8, 256), 256, 0, (cudaStream_t)stream>>>((const unsigned short*)a, (const unsigned short*)b, (unsigned short*)out, n_elems / 8,
-                                                                                   act_dtype == B2T_ACT_F16);
+    B2T_LAUNCH(add_relu_kernel, grid_for(n_elems / 8, 256), 256, 0, (cudaStream_t)stream, (const unsigned short*)a, (const unsigned short*)b, (unsigned short*)out,
+               n_elems / 8, act_dtype == B2T_ACT_F16);
     return rcheck("add_relu");
 }
 
 extern "C" int b2t_avgpool_l2norm(const void* in, float* out, int n, int hw, int c, int act_dtype, void* stream) {
     if (!in || !out || n < 1 || hw < 1 || c != 512) return rfail(B2T_EINVAL, "b2t_avgpool_l2norm: 512 channels expected");
-    avgpool_l2norm_kernel<<<n, 128, 0, (cudaStream_t)stream>>>((const unsigned short*)in, out, hw, act_dtype == B2T_ACT_F16);
+    B2T_LAUNCH(avgpool_l2norm_kernel, n, 128, 0, (cudaStream_t)stream, (const unsigned short*)in, out, hw, act_dtype == B2T_ACT_F16);
     return rcheck("avgpool_l2norm");
 }

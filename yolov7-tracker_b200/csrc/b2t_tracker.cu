@@ -30,7 +30,7 @@ static int check_launch(const char* what) {
     return B2T_OK;
 }
 extern "C" const char* b2t_last_error(void) { return g_err.c_str(); }
-extern "C" int b2t_version(void) { return 101; }
+extern "C" int b2t_version(void) { return 102; }
 extern "C" long long b2t_launch_count(void) { return g_launches; }
 
 // ------------------------------------------------------------------------------------------ Kalman kernels

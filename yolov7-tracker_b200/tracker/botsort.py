@@ -133,6 +133,8 @@ class BoTSORT(BaseTracker):
         crops = []
         for tlbr in tlbrs:
             x1, y1, x2, y2 = list(map(int, tlbr))
+            if min(x1, y1, x2, y2) < 0:                                        # the slice would wrap to the far side of the frame
+                raise L.B2TError("get_feature: a box has a negative coordinate after int() (clip the boxes to the frame first)")
             crops.append(img[y1:y2, x1:x2])
         return self.reid_model(crops)
 
