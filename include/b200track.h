@@ -330,6 +330,37 @@ int b2t_batchnorm_batch_stats(const void* x, void* y, long long n_pix, int c, co
 /* nn.AvgPool2d over the whole hw-position map (:83) + division by the L2 norm (:103-104): in [n][hw][512] -> out [n][512] fp32 */
 int b2t_avgpool_l2norm(const void* in, float* out, int n, int hw, int c, int act_dtype, void* stream);
 
+/* ---- appearance for many sequences in one extractor pass (TrackingPipeline with ReID).  The reference builds one tracker per sequence
+ * (tracker/track.py:123,132); each BoTSORT.update crops that sequence's det_high rows (botsort.py:339-346, :291-311) and calls the
+ * extractor on them alone, so every BatchNorm normalises with that sequence's crops (the net is never put in eval(), q16).
+ * b2t_reid_crops_from_dets: the crop list of all sequences, built on the device from the NMS output.
+ *   dets [n_seq][dmax][6] (x1, y1, x2, y2, score, cls, after scale_coords + clip + round) and det_count [n_seq]; det_thresh as the tracker
+ *   takes it ((float)conf_thresh, b2t_tracker.cu).  Per sequence, the rows i < det_count[s] with score >= det_thresh in row order (the
+ *   tracker's det_high test, without its has_area filter: the reference crops every det_high row) become the crops
+ *   frame_s[int(y1):int(y2), int(x1):int(x2)] (int() truncates, right / bottom ends clipped to the height x width frame) of the
+ *   (n_seq, height, width, 3) uint8 buffer, as b2t_reid_crops descriptors, sequence-major:
+ *     crops   [cap][4]     {byte offset into the buffer, row pitch 3 * width, height, width}; rows [offsets[n_seq], cap) repeat crop 0
+ *                          (a 1 x 1 crop of frame 0 when there is none), so b2t_reid_crops over all cap rows reads valid pixels
+ *     offsets [n_seq + 1]  segment s = crops [offsets[s], offsets[s + 1]) (clamped to cap)
+ *     rowmap  [cap]        crop j -> feature row s * dmax + i of the tracker's [n_seq][dmax][feat] buffer; -1 for padding
+ *     status  [n_seq + 1]  status[s] = B2T_REID_* bits of sequence s; status[n_seq] = det_high rows of all sequences (uncapped)
+ *   A refused row (zero size / negative coordinate) gets a 1 x 1 descriptor and its bit; a row past cap is dropped with
+ *   B2T_REID_OVERFLOW.  One launch, no host synchronisation. */
+enum { B2T_REID_OVERFLOW = 1,    /* more det_high rows than cap */
+       B2T_REID_ZERO_SIZE = 2,   /* an empty crop: the reference prints "size in bbox exists zero" and exits (deepsort_reid.py:141-142) */
+       B2T_REID_NEGATIVE = 4 };  /* a coordinate < 0 after int() (or NaN): the reference's slice would wrap to the far side of the frame */
+int b2t_reid_crops_from_dets(const float* dets, const int* det_count, int n_seq, int dmax, float det_thresh, int height, int width, int cap,
+                             long long* crops, int* offsets, int* rowmap, int* status, void* stream);
+/* b2t_batchnorm_batch_stats per segment: x [max_crops][pix_per_crop][c], segment s = crops [offsets[s], offsets[s + 1]) (device offsets,
+ * non-decreasing, offsets[n_seg] <= max_crops).  Each segment's output is bitwise that of b2t_batchnorm_batch_stats on the segment
+ * alone (same block partition, shift, tree and summation order); empty segments and the rows past offsets[n_seg] are not touched.
+ * ws: device scratch of b2t_batchnorm_segments_workspace_bytes(n_seg, max_crops, pix_per_crop, c) bytes.  In place is allowed. */
+size_t b2t_batchnorm_segments_workspace_bytes(int n_seg, int max_crops, int pix_per_crop, int c);   /* 0 for refused arguments */
+int b2t_batchnorm_batch_stats_segments(const void* x, void* y, const int* offsets, int n_seg, int max_crops, int pix_per_crop, int c,
+                                       const float* gamma, const float* beta, float eps, int relu, double* ws, int act_dtype, void* stream);
+/* b2t_avgpool_l2norm with crop j written to row rowmap[j] of out [rows][512] (:83, :103-104); rowmap[j] < 0: nothing written */
+int b2t_avgpool_l2norm_rows(const void* in, float* out, const int* rowmap, int n, int hw, int c, int act_dtype, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -15,6 +15,7 @@ FMT_XYAH, FMT_XYWH, FMT_NSA = 0, 1, 2
 SORT, BYTETRACK, BOTSORT = 0, 1, 2
 FLAG_MEAN_F32, FLAG_NOT_TRACKED = 1, 2
 ACT_BF16, ACT_F16 = 0, 1
+REID_OVERFLOW, REID_ZERO_SIZE, REID_NEGATIVE = 1, 2, 4       # b2t_reid_crops_from_dets status bits
 OUT_COLS, STAT_WORDS, STAT_PHASE0, STAT_SUB0 = 8, 64, 16, 32
 STAT_NAPP, STAT_NAPPLOW = 30, 31          # appearance pairs, and those whose cost the appearance lowered
 GMC_STAT_WORDS, GMC_FIRST_FRAME, GMC_FEW_POINTS, GMC_TRUNCATED = 8, 1, 2, 4
@@ -104,6 +105,10 @@ SIGNATURES = {
     "b2t_batchnorm_workspace_bytes": (_SZ, [C.c_longlong, _I]),
     "b2t_batchnorm_batch_stats": (_I, [_P, _P, C.c_longlong, _I, _P, _P, C.c_float, _I, _P, _I, _P]),
     "b2t_avgpool_l2norm": (_I, [_P, _P, _I, _I, _I, _I, _P]),
+    "b2t_reid_crops_from_dets": (_I, [_P, _P, _I, _I, C.c_float, _I, _I, _I, _P, _P, _P, _P, _P]),
+    "b2t_batchnorm_segments_workspace_bytes": (_SZ, [_I, _I, _I, _I]),
+    "b2t_batchnorm_batch_stats_segments": (_I, [_P, _P, _P, _I, _I, _I, _I, _P, _P, C.c_float, _I, _P, _I, _P]),
+    "b2t_avgpool_l2norm_rows": (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
     "b2t_detect_nms": (_I, [_P, _I, _I, _I, C.c_float, C.c_float, _I, _I, _I, _I, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,
                             _P, _SZ, _P, _P, _P]),
 }
@@ -121,7 +126,8 @@ NMS_SYMBOLS = ["b2t_detect_last_error", "b2t_nms_workspace_bytes", "b2t_nms", "b
 
 # the appearance branch's element-wise kernels (csrc/b2t_reid.cu) also compile for the host simulator
 REID_SYMBOLS = ["b2t_reid_crops", "b2t_maxpool3x3s2", "b2t_maxpool2x2s2", "b2t_add_relu", "b2t_batchnorm_workspace_bytes", "b2t_batchnorm_batch_stats",
-                "b2t_avgpool_l2norm"]
+                "b2t_avgpool_l2norm", "b2t_reid_crops_from_dets", "b2t_batchnorm_segments_workspace_bytes", "b2t_batchnorm_batch_stats_segments",
+                "b2t_avgpool_l2norm_rows"]
 
 # the association branch (csrc/b2t_tracker.cu); the rest are the detector's translation units
 TRACKER_SYMBOLS = [n for n in SIGNATURES if not n.startswith(("b2t_conv", "b2t_detect", "b2t_image", "b2t_upsample", "b2t_spp", "b2t_nms", "b2t_letterbox", "b2t_gmc_workspace", "b2t_gmc_reset", "b2t_gmc_estimate", "b2t_gmc_prepare",

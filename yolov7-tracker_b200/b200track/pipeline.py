@@ -11,6 +11,9 @@ detectors (same weights, same plans, own buffers; frames alternate between them)
 post-processed while frame t's forward runs: the detect stream never idles between forward graphs.  Cross-frame hazards (the input
 staging, the stem input, the head maps and the NMS output of each detector) are guarded by events.  ``step()`` returns the tracks of
 the PREVIOUS call (one frame of latency, same results); ``flush()`` returns the last ones.
+With ``reid=`` (BoT-SORT with appearance) the tracker stream also builds the crop list of every sequence's det_high rows from the NMS
+output, cuts the crops out of the detector's uint8 frame buffer (after which the next copy may overwrite it), runs the extractor's graph
+with BatchNorm statistics per sequence, and hands the features to the tracker step -- no host round trip.
 """
 import torch
 
@@ -18,11 +21,16 @@ from . import _lib as L
 
 
 class TrackingPipeline:
-    def __init__(self, detector, engine, out_rows=512, gmc=None):
+    def __init__(self, detector, engine, out_rows=512, gmc=None, reid=None, reid_cap=None):
         """detector: a ``DetectorW6`` or a pair of twins (see above).
         gmc: a ``b200track.gmc.GmcEstimator`` for the source-frame size (BoT-SORT with camera-motion compensation, reference
         botsort.py:380-382): the warp of every sequence is estimated on the GPU from the uint8 frames and the NMS output and fed
-        to the tracker step without leaving the device."""
+        to the tracker step without leaving the device.
+        reid: a ``b200track.reid.ReidExtractor`` (BoT-SORT with appearance, reference botsort.py:339-349; the engine must be BoT-SORT
+        with feat_dim = 512): one extractor pass per step over the det_high crops of all sequences, each sequence's crops normalised
+        with its own batch statistics as the reference's one-tracker-per-sequence calls do.  reid_cap: crops per pass (default
+        n_seq * dmax, which cannot overflow); a step with more det_high rows raises B2TError when its tracks are collected.
+        Frames must then be uint8 (the crops come from det.src_u8)."""
         self.dets = list(detector) if isinstance(detector, (list, tuple)) else [detector]
         if len(self.dets) not in (1, 2):
             raise L.B2TError("TrackingPipeline takes one detector or two twins")
@@ -36,6 +44,21 @@ class TrackingPipeline:
             raise L.B2TError("GmcEstimator(n_seq=%d) does not match DetectorW6(batch=%d)" % (gmc.S, det.B))
         dev = det.dev
         self.dev = dev
+        self.reid, self.reid_net = reid, None
+        if reid is not None:
+            if engine.kind != "botsort" or engine.feat_dim != 512:
+                raise L.B2TError("TrackingPipeline(reid=): the engine must be BoT-SORT with feat_dim=512 (got %s, feat_dim=%d)" % (engine.kind, engine.feat_dim))
+            idx = lambda d: torch.device(d).index if torch.device(d).index is not None else torch.cuda.current_device()      # noqa: E731
+            if not (idx(reid.dev) == idx(dev) == idx(engine.device)):
+                raise L.B2TError("TrackingPipeline(reid=): extractor on %s, detector on %s, engine on %s" % (reid.dev, dev, engine.device))
+            cap = engine.S * engine.dmax if reid_cap is None else int(reid_cap)
+            if cap < 1:
+                raise L.B2TError("TrackingPipeline: reid_cap must be >= 1, got %d" % cap)
+            self.reid_net = reid.segmented(engine.S, engine.dmax, cap)
+            self.reid_net.capture()
+            self.h_rstat = [torch.zeros(engine.S + 1, dtype=torch.int32).pin_memory() for _ in range(2)]
+        elif reid_cap is not None:
+            raise L.B2TError("TrackingPipeline: reid_cap without reid")
         self.twin = len(self.dets) == 2
         self.s_copy, self.s_det, self.s_trk = (torch.cuda.Stream(device=dev) for _ in range(3))
         self.s_nms = torch.cuda.Stream(device=dev) if self.twin else self.s_det
@@ -87,6 +110,8 @@ class TrackingPipeline:
         i = k if self.twin else 0
         det = self.dets[i]
         u8 = frames.dtype == torch.uint8
+        if self.reid is not None and not u8:
+            raise L.B2TError("TrackingPipeline(reid=): frames must be uint8 BGR (the crops are cut from det.src_u8), got %s" % frames.dtype)
         if u8 and (getattr(det, "src_u8", None) is None or tuple(frames.shape) != tuple(det.src_u8.shape)):
             raise L.B2TError("uint8 frames of shape %s: call det.set_source_frames((h, w)) first" % (tuple(frames.shape),))
         # ---- input: copy once the previous ingest of this detector has read the staging buffer; the ingest kernel follows on the same
@@ -110,7 +135,8 @@ class TrackingPipeline:
                     self.gmc.prepare(det.src_u8, k)                            # gray / FAST scores / smoothed image while the frame buffer is valid
             else:
                 det.ops[0][0]()                                                # ReOrg + 16-bit NHWC of the float tensor
-            self.ev_src_free[i].record(s_in)
+            if self.reid is None:
+                self.ev_src_free[i].record(s_in)                               # (with ReID: once the crops have been cut, below)
             if self.twin:
                 self.ev_in_ready[i].record(s_in)
         # ---- detect
@@ -129,14 +155,25 @@ class TrackingPipeline:
         # ---- associate + read back
         with torch.cuda.stream(self.s_trk):
             self.s_trk.wait_event(self.ev_nms_done[i])
+            rn = self.reid_net
+            if rn is not None:
+                # crop list of every sequence's det_high rows + the crops cut out of the frames: det.src_u8 is free after this
+                rn.cut(det.src_u8, det.out, det.out_count, float(eng.cfg.conf_thresh))
+                self.ev_src_free[i].record(self.s_trk)
             if self.gmc is not None and u8:
                 # key points outside the boxes of the high-score detections (botsort.py:380), matching, RANSAC -> warps on the device
                 w23, _ = self.gmc.estimate_prepared(k, det.out, det.out_count, det_thresh=float(eng.cfg.conf_thresh))
                 warps = w23.view(eng.S, 6)
-            eng.step_device(det.out, det.out_count, self.t_out, self.t_stat, warps=warps)
+            if rn is not None:
+                rn.run()                                                       # extractor graph -> rn.feats rows s * dmax + i
+                eng.step_device(det.out, det.out_count, self.t_out, self.t_stat, warps=warps, feats=rn.feats)
+            else:
+                eng.step_device(det.out, det.out_count, self.t_out, self.t_stat, warps=warps)
             self.ev_out_free[i].record(self.s_trk)
             self.h_out[k].copy_(self.t_out, non_blocking=True)
             self.h_stat[k].copy_(self.t_stat, non_blocking=True)
+            if rn is not None:
+                self.h_rstat[k].copy_(rn.status, non_blocking=True)
             self.ev_trk_done[k].record(self.s_trk)
         self.n += 1
         if self.n == 1:
@@ -148,6 +185,8 @@ class TrackingPipeline:
         err = int(self.h_stat[k][:, L.STAT_ERR].max())
         if err:
             raise L.B2TError("tracker capacity error bits 0x%x (slots / detections / edges / output rows)" % err)
+        if self.reid_net is not None:
+            self.reid_net.raise_for_status(self.h_rstat[k].numpy())
         return self.h_out[k], self.h_stat[k]
 
     def flush(self):

@@ -5,6 +5,8 @@ ReLU + max-pool, four stages of two ``BasicBlock``s (:14-49), 8 x 4 average pool
 64 x 128 pixels: the 20 convolutions (+ folded BatchNorm + ReLU) are plans of the wgmma conv kernel (csrc/b2t_conv.cu, act = 2),
 the crop / resize / normalise step, the max-pool, the residual add + ReLU and the average pool + norm are the element-wise kernels of
 csrc/b2t_reid.cu.  NHWC fp16 activations, fp32 accumulation -- the same numerics as the detector branch.
+``ReidExtractor.segmented`` is the same network over the det_high crops of MANY sequences in one pass, with every batch-statistics
+BatchNorm normalising each sequence's crops with that sequence's statistics alone (``SegmentedReid``, used by ``TrackingPipeline``).
 Weights: the ``net_dict`` of the reference's checkpoint (weights/ckpt.t7), or any state dict with the same keys.
 """
 import ctypes as C
@@ -91,8 +93,9 @@ class ReidExtractor:
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
 
-    def _build(self, n):
-        """Buffers and conv plans for a batch of n crops."""
+    def _build(self, n, seg=None):
+        """Buffers and conv plans for a batch of n crops.  seg (a SegmentedReid): BatchNorm statistics per segment of seg.offsets and
+        the pooled features of crop j to row seg.rowmap[j] of seg.feats."""
         dev, dt = self.dev, self.dtype
         buf = lambda h, w, c: torch.zeros((n, h, w, c), dtype=dt, device=dev)          # noqa: E731
         net = {"n": n, "valid": n, "x": buf(128, 64, 16), "c0": buf(128, 64, 64), "ops": []}
@@ -113,6 +116,13 @@ class ReidExtractor:
             if batch:
                 g, beta = self.bn[name]
                 ho, wo = h // s, w // s
+                if seg is not None:
+                    bn_bytes[0] = max(bn_bytes[0], int(self.lib.b2t_batchnorm_segments_workspace_bytes(seg.S, n, ho * wo, cout)))
+                    # statistics per sequence (segment), the padding crops past offsets[S] excluded
+                    ops.append(lambda y=y, g=g, beta=beta, c=cout, hw=ho * wo, relu=int(act == 2): check(self.lib.b2t_batchnorm_batch_stats_segments(
+                        y.data_ptr(), y.data_ptr(), seg.offsets.data_ptr(), seg.S, n, hw, c, g.data_ptr(), beta.data_ptr(), EPS, relu,
+                        bn_ws[0].data_ptr(), self.code, self._stream())))
+                    return plan
                 bn_bytes[0] = max(bn_bytes[0], int(self.lib.b2t_batchnorm_workspace_bytes(n * ho * wo, cout)))     # grows with n_pix
                 # statistics over the VALID crops only (net["valid"]): the rows that pad the batch to its capacity must not count
                 ops.append(lambda y=y, g=g, beta=beta, c=cout, hw=ho * wo, relu=int(act == 2): check(self.lib.b2t_batchnorm_batch_stats(
@@ -140,9 +150,13 @@ class ReidExtractor:
                 cur, h, w = out, ho, wo
         if self.bn_mode == "batch":
             bn_ws[0] = net["bn_ws"] = torch.zeros((bn_bytes[0] + 7) // 8, dtype=torch.float64, device=dev)
-        net["feat"] = torch.zeros((n, 512), dtype=torch.float32, device=dev)
         last = cur
-        ops.append(lambda a=last, o=net["feat"]: check(self.lib.b2t_avgpool_l2norm(a.data_ptr(), o.data_ptr(), n, h * w, 512, self.code, self._stream())))
+        if seg is not None:
+            ops.append(lambda a=last: check(self.lib.b2t_avgpool_l2norm_rows(a.data_ptr(), seg.feats.data_ptr(), seg.rowmap.data_ptr(), n, h * w, 512,
+                                                                              self.code, self._stream())))
+        else:
+            net["feat"] = torch.zeros((n, 512), dtype=torch.float32, device=dev)
+            ops.append(lambda a=last, o=net["feat"]: check(self.lib.b2t_avgpool_l2norm(a.data_ptr(), o.data_ptr(), n, h * w, 512, self.code, self._stream())))
         net["flops"] = sum(p.flops for p in net["plans"])
         net["launches"] = len(ops) + 1
         return net
@@ -155,6 +169,37 @@ class ReidExtractor:
             with torch.cuda.device(self.dev):
                 self._nets[cap] = self._build(cap)
         return self._nets[cap]
+
+    def segmented(self, n_seq, dmax, cap=None):
+        """The network over the det_high crops of n_seq sequences at once, at a fixed capacity of cap crops (default n_seq * dmax,
+        which cannot overflow): see SegmentedReid."""
+        return SegmentedReid(self, n_seq, dmax, n_seq * dmax if cap is None else cap)
+
+    def features_segments(self, frames, tlbrs_per_seq, cap=None):
+        """Host-facing form of the segmented pass (tests, tools): frames (S, H, W, 3) uint8 BGR, tlbrs_per_seq: per sequence an
+        (n_s, 4) array of boxes.  Returns per sequence the (n_s, 512) features -- each sequence's crops normalised with its own batch
+        statistics, as ``features_from_frame(frames[s], tlbrs_per_seq[s])`` alone computes them.  Raises B2TError for a refused crop."""
+        import numpy as np
+        f = frames if isinstance(frames, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(frames))
+        f = f.to(self.dev).contiguous()
+        S = int(f.shape[0])
+        if len(tlbrs_per_seq) != S:
+            raise L.B2TError("features_segments: %d box lists for %d frames" % (len(tlbrs_per_seq), S))
+        boxes = [np.asarray(t, dtype=np.float32).reshape(-1, 4) for t in tlbrs_per_seq]
+        dmax = max(1, max(len(b) for b in boxes))
+        dets = np.zeros((S, dmax, 6), np.float32)
+        for s, b in enumerate(boxes):
+            dets[s, :len(b), :4] = b
+            dets[s, :len(b), 4] = 1.0
+        seg = self.segmented(S, dmax, cap)
+        d_dets = torch.from_numpy(dets).to(self.dev)
+        d_cnt = torch.tensor([len(b) for b in boxes], dtype=torch.int32, device=self.dev)
+        with torch.cuda.device(self.dev):
+            seg.cut(f, d_dets, d_cnt, 0.5)
+            seg.run()
+            status = seg.status.cpu().numpy()
+        seg.raise_for_status(status)
+        return [seg.feats[s, :len(b)].clone() for s, b in enumerate(boxes)]
 
     def features(self, pixels, crops):
         """pixels: uint8 device tensor holding BGR pixels (a batch of frames, or crops packed back to back); crops: (n, 4) int64 rows
@@ -209,3 +254,88 @@ class ReidExtractor:
             o += h * w * 3
         pixels = torch.from_numpy(np.concatenate(offs)).to(self.dev)
         return self.features(pixels, torch.tensor(rows, dtype=torch.int64)).cpu().numpy()
+
+
+class SegmentedReid:
+    """The extractor over the det_high crops of S sequences in ONE pass, at a fixed capacity of `cap` crops, with nothing in a step that
+    depends on a host-side count: the crop descriptors, segment offsets and row map are device tensors written by
+    b2t_reid_crops_from_dets from the NMS output.  ``cut`` (two launches) builds the crop list and cuts the crops out of the frames, after
+    which the frame buffer may be overwritten; ``run`` replays one CUDA graph of the 20 convs, the BatchNorms (statistics per sequence in
+    batch mode, b2t_batchnorm_batch_stats_segments; folded in running mode), pools and adds, and writes the features of crop j to row
+    rowmap[j] of ``feats`` (S, dmax, 512) -- the tensor TrackEngine.step_device(feats=) takes.  Padding crops cost full compute and go
+    nowhere."""
+
+    def __init__(self, ext, n_seq, dmax, cap):
+        if n_seq < 1 or dmax < 1 or cap < 1:
+            raise L.B2TError("SegmentedReid: n_seq, dmax and cap must be >= 1 (got %d, %d, %d)" % (n_seq, dmax, cap))
+        self.ext, self.S, self.dmax, self.cap = ext, int(n_seq), int(dmax), int(cap)
+        dev = ext.dev
+        with torch.cuda.device(dev):
+            self.crops = torch.zeros((self.cap, 4), dtype=torch.int64, device=dev)
+            self.offsets = torch.zeros(self.S + 1, dtype=torch.int32, device=dev)
+            self.rowmap = torch.full((self.cap,), -1, dtype=torch.int32, device=dev)
+            self.status = torch.zeros(self.S + 1, dtype=torch.int32, device=dev)
+            self.feats = torch.zeros((self.S, self.dmax, 512), dtype=torch.float32, device=dev)
+            self.net = ext._build(self.cap, seg=self)
+        self.graph = None
+        self.bytes = sum(t.numel() * t.element_size() for t in self._tensors())
+
+    def _tensors(self):
+        net = self.net
+        ts = [self.crops, self.offsets, self.rowmap, self.status, self.feats, net["x"], net["c0"]] + net.get("keep", [])
+        if "bn_ws" in net:
+            ts.append(net["bn_ws"])
+        seen, out = set(), []
+        for t in ts:
+            if t.data_ptr() not in seen:
+                seen.add(t.data_ptr()); out.append(t)
+        return out
+
+    def cut(self, frames, dets, det_count, det_thresh):
+        """On the current stream: frames (S, H, W, 3) uint8 device tensor, dets (S, dmax, 6) float32, det_count (S,) int32 (the
+        detector's out / out_count); det_thresh: the tracker's conf_thresh (compared in float32)."""
+        ext = self.ext
+        if tuple(dets.shape) != (self.S, self.dmax, 6) or dets.dtype != torch.float32 or det_count.dtype != torch.int32 or tuple(det_count.shape) != (self.S,):
+            raise L.B2TError("SegmentedReid.cut: dets must be float32 (%d, %d, 6) and det_count int32 (%d,)" % (self.S, self.dmax, self.S))
+        if frames.dtype != torch.uint8 or frames.dim() != 4 or int(frames.shape[0]) != self.S or int(frames.shape[3]) != 3 or not frames.is_contiguous():
+            raise L.B2TError("SegmentedReid.cut: frames must be a contiguous uint8 (%d, H, W, 3) tensor" % self.S)
+        H, W = int(frames.shape[1]), int(frames.shape[2])
+        rc = ext.lib.b2t_reid_crops_from_dets(dets.data_ptr(), det_count.data_ptr(), self.S, self.dmax, float(det_thresh), H, W, self.cap,
+                                              self.crops.data_ptr(), self.offsets.data_ptr(), self.rowmap.data_ptr(), self.status.data_ptr(), ext._stream())
+        if rc == 0:
+            rc = ext.lib.b2t_reid_crops(frames.data_ptr(), self.crops.data_ptr(), self.cap, self.net["x"].data_ptr(), ext.code, ext._stream())
+        if rc != 0:
+            raise L.B2TError("SegmentedReid.cut: %s" % (ext.lib.b2t_detect_last_error() or b"").decode())
+
+    def run(self):
+        """On the current stream: the network on the cut crops -> feats (one CUDA graph; captured on the first call)."""
+        if self.graph is None:
+            self.capture()
+        self.graph.replay()
+
+    def capture(self):
+        """Capture the graph of ``run`` (synchronises the device).  The ops read only device tensors, so capturing before any ``cut``
+        is safe: the warm-up normalises nothing (empty segments) and writes no feature row (row map all -1)."""
+        cur = torch.cuda.current_stream(self.ext.dev)
+        cs = torch.cuda.Stream(device=self.ext.dev)              # captured on a side stream (the current one may be the legacy default)
+        cs.wait_stream(cur)
+        with torch.cuda.device(self.ext.dev), torch.cuda.stream(cs):
+            for op in self.net["ops"]:                           # warm-up outside the capture (module loading)
+                op()
+        cs.synchronize()
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph, stream=cs):
+            for op in self.net["ops"]:
+                op()
+        cur.wait_stream(cs)
+
+    def raise_for_status(self, status):
+        """status: the (S + 1,) status words read back (host array) -> B2TError naming the first refused condition and sequence."""
+        for s in range(self.S):
+            bits = int(status[s])
+            if bits & L.REID_OVERFLOW:
+                raise L.B2TError("ReID: sequence %d: the det_high crops of this step (%d in all sequences) exceed reid_cap = %d" % (s, int(status[self.S]), self.cap))
+            if bits & L.REID_ZERO_SIZE:
+                raise L.B2TError("ReID: sequence %d: a det_high box gives a crop of zero size (the reference prints 'size in bbox exists zero' and exits)" % s)
+            if bits & L.REID_NEGATIVE:
+                raise L.B2TError("ReID: sequence %d: a det_high box has a negative coordinate after int() (the reference's slice would wrap)" % s)
