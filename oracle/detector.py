@@ -28,14 +28,18 @@ def _bf(t, on):
     return t.to(torch.bfloat16 if on is True else on).float()
 
 
-def forward(layers, sd, img, anchors, strides, nc=80, emulate_bf16=False, return_raw=False, act="silu", name_offset=0):
+def forward(layers, sd, img, anchors, strides, nc=80, emulate_bf16=False, return_raw=False, act="silu", name_offset=0, return_layers=False):
     """img (B,3,H,W) float32 in [0,1] -> pred (B, N, 5+nc) as ``model(img)[0]`` of the fused reference model.
     act: "silu" (w6, models/common.py:105) or "leaky" (YOLOv7-tiny: nn.LeakyReLU(0.1), cfg/deploy/yolov7-tiny.yaml:15);
-    name_offset: layer index -> the reference's module index (the tiny layer list carries an explicit input op in front: -1)."""
+    name_offset: layer index -> the reference's module index (the tiny layer list carries an explicit input op in front: -1).
+    return_layers: return dict(pred, layers = every layer's output by index (None for Detect), spp = {layer index: the SPPCSPC
+    temporaries t1 (cv1), t2 (cv3), x1 (cv4), m5 / m9 / m13 (pools of x1), t5 (cv5), y1 (cv6), y2 (cv2)}, raw = the Detect
+    convs' (B, 3 * no, h, w) outputs per level) -- a chain of stored layer outputs to check a per-layer harness against."""
     no = nc + 5
     no_ = name_offset
     dev = img.device
     y = []
+    spp = {}
 
     def conv(name, x, k, s, act=True):
         w = _bf(sd[name + ".weight"].to(dev).float(), emulate_bf16)
@@ -67,15 +71,20 @@ def forward(layers, sd, img, anchors, strides, nc=80, emulate_bf16=False, return
         elif op == "sppcspc":
             xin = y[_r(i, frm)]
             p = "model.%d." % (i + no_)
-            x1 = conv(p + "cv4.conv", conv(p + "cv3.conv", conv(p + "cv1.conv", xin, 1, 1), 3, 1), 1, 1)
+            t1 = conv(p + "cv1.conv", xin, 1, 1)
+            t2 = conv(p + "cv3.conv", t1, 3, 1)
+            x1 = conv(p + "cv4.conv", t2, 1, 1)
             pools = [F.max_pool2d(x1, k, 1, k // 2) for k in (5, 9, 13)]
-            y1 = conv(p + "cv6.conv", conv(p + "cv5.conv", torch.cat([x1] + pools, 1), 1, 1), 3, 1)
+            t5 = conv(p + "cv5.conv", torch.cat([x1] + pools, 1), 1, 1)
+            y1 = conv(p + "cv6.conv", t5, 3, 1)
             y2 = conv(p + "cv2.conv", xin, 1, 1)
             out = conv(p + "cv7.conv", torch.cat((y1, y2), 1), 1, 1)
+            spp[i] = dict(t1=t1, t2=t2, x1=x1, m5=pools[0], m9=pools[1], m13=pools[2], t5=t5, y1=y1, y2=y2)
         elif op == "detect":
-            z, raws = [], []
+            z, raws, maps = [], [], []
             for lvl, f in enumerate(frm):
                 r = conv("model.%d.m.%d" % (i + no_, lvl), y[f], 1, 1, act=False)
+                maps.append(r)
                 bs, _, ny, nx = r.shape
                 r = r.view(bs, 3, no, ny, nx).permute(0, 1, 3, 4, 2).contiguous()
                 raws.append(r)
@@ -87,6 +96,8 @@ def forward(layers, sd, img, anchors, strides, nc=80, emulate_bf16=False, return
                 s[..., 2:4] = (s[..., 2:4] * 2) ** 2 * a
                 z.append(s.view(bs, -1, no))
             pred = torch.cat(z, 1)
+            if return_layers:
+                return dict(pred=pred, layers=y + [None], spp=spp, raw=maps)
             return (pred, raws) if return_raw else pred
         y.append(out)
     raise RuntimeError("layer list has no detect layer")

@@ -41,14 +41,17 @@ class RecorderLib:
         return fn
 
 
-def dry_run_plan(batch, img_size, **kw):
-    """Returns (detector, [per-conv dict]) for a plan built on CPU tensors.  Pointers are reported relative to their tensors."""
+def dry_run_plan(batch, img_size, tiny=False, **kw):
+    """Returns (detector, [per-conv dict]) for a plan built on CPU tensors.  Pointers are reported relative to their tensors.
+    tiny: plan the YOLOv7-tiny graph (``b200track.tiny.DetectorTiny``) instead of w6."""
     from b200track import _lib as L
     from b200track import detector as D
+    from b200track import tiny as T
     from b200track.w6 import seeded_state_dict
     rec = RecorderLib()
+    make = (lambda **a: T.DetectorTiny(T.seeded_state_dict(0), **a)) if tiny else (lambda **a: D.DetectorW6(seeded_state_dict(0), **a))
     with mock.patch.object(L, "load", lambda: rec), mock.patch.object(torch.cuda, "is_available", lambda: True):
-        det = D.DetectorW6(seeded_state_dict(0), batch=batch, img_size=img_size, device="cpu", use_graph=False, autotune=False, **kw)
+        det = make(batch=batch, img_size=img_size, device="cpu", use_graph=False, autotune=False, **kw)
     # run every op once against the recorder: the scalar arguments of each C-ABI call become part of the plan
     rec.launches = []
 

@@ -155,6 +155,7 @@ class DetectorW6:
         lib = self.lib
         stream = lambda: C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)  # noqa: E731
         self.raw, self.decode_ops = [], []
+        self.spp_tmp = {}               # SPPCSPC layer index -> its temporaries: t1 (cv1), t2 (cv3), cat4 = [cv4 | m5 | m9 | m13], t5 (cv5), cat2 = [cv6 | cv2]
         levels = []
         fused_away = set()
         pairs = set(stackable_pairs(layers)) if fuse_pairs else set()
@@ -205,6 +206,7 @@ class DetectorW6:
                 c_ = c2
                 t1, t2 = new_buf(h, c_), new_buf(h, c_)
                 cat4, t5, cat2 = new_buf(h, 4 * c_), new_buf(h, c_), new_buf(h, 2 * c_)
+                self.spp_tmp[i] = dict(t1=t1, t2=t2, cat4=cat4, t5=t5, cat2=cat2)      # read-only record, for per-layer checks
                 pre = "model.%d." % (i + no_)
                 conv_op(pre + "cv1.conv", place[j], c1, (t1, 0), c_, 1, 1, h)
                 conv_op(pre + "cv3.conv", (t1, 0), c_, (t2, 0), c_, 3, 1, h)
