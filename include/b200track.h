@@ -235,9 +235,10 @@ int b2t_detect_decode(const float* raw, int raw_pitch, float* pred, int B, int H
                       long long n_total, float stride, const float* anchors_host, void* stream);
 /* utils/general.py:607-695 non_max_suppression (best-class path, class-offset boxes, torchvision.ops.nms greedy rule,
  * max_nms cap, max_det cap; csrc/b2t_nms.cu).  pred [B][N][no] fp32 -> out [B][max_det][6] (x1 y1 x2 y2 conf cls),
- * out_count [B]; rows >= out_count[b] are not written.  post != 0 also applies scale_coords (gain, pad) + clip to
- * (img_w, img_h) + round (tracker/track.py:239-240).  0 <= conf_thres, max_det <= 2048, max_cand bounds the rows
- * that may pass the filter (extra ones are dropped: size it N to be exact). */
+ * out_count [B]; rows >= out_count[b] are not written.  post != 0 also applies scale_coords (gain > 0, pad) + clip to
+ * (img_w, img_h) + round (tracker/track.py:239-240) -- x - pad and a multiply by the fp32 reciprocal of gain, which is
+ * what torch computes for that line on a CUDA tensor.  0 <= conf_thres, max_det <= 2048, max_cand >= N (every row may
+ * pass the filter; a smaller value is refused with B2T_EINVAL). */
 size_t b2t_nms_workspace_bytes(int B, int max_cand, int max_nms);
 int b2t_nms(const float* pred, int B, int N, int no, float conf_thres, float iou_thres, int max_det, int max_nms, int max_cand,
             int post, float gain, float padw, float padh, float img_w, float img_h, void* workspace, size_t workspace_bytes,
@@ -246,7 +247,7 @@ int b2t_nms(const float* pred, int B, int N, int no, float conf_thres, float iou
  * what `non_max_suppression(model(img)[0], conf_thres, iou_thres)` returns, computed from the raw head maps without
  * materialising the (B, N, no) prediction tensor.  Level k: raw [B][h][w][raw_pitch] fp32 (channel a*no + o, 3 anchors),
  * anchors = (w,h) x 3 in pixels, level_off = first prediction row of the level (rows (a*h + y)*w + x follow).  Same
- * workspace, outputs and limits as b2t_nms. */
+ * workspace, outputs and limits as b2t_nms; max_cand >= the rows per image, 3 h w summed over the levels. */
 typedef struct b2t_head_level {
     const float* raw;
     int raw_pitch, h, w;

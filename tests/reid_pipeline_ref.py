@@ -136,10 +136,11 @@ def run_pool_rows(lib, be, x, rowmap, n_rows, hw, dt):
 def widen_degenerate(dets, size):
     """The seeded random-init detector emits boxes that round to zero width or height at score 1.0 (the reference's own note at
     botsort.py:283, "why some bboxs has 0 area"); the reference exits on such a det_high crop, and no threshold avoids them.  Tests
-    that need a stream of valid crops widen every box to at least 2 px inside the size x size frame, in place on the current stream,
-    identically in every arm they compare."""
-    x1 = dets[..., 0].clamp(max=size - 2)
-    y1 = dets[..., 1].clamp(max=size - 2)
+    that need a stream of valid crops widen every box to at least 2 px inside the frame (size: its side, or its (height, width)),
+    in place on the current stream, identically in every arm they compare."""
+    h, w = (size, size) if isinstance(size, int) else size
+    x1 = dets[..., 0].clamp(max=w - 2)
+    y1 = dets[..., 1].clamp(max=h - 2)
     dets[..., 0] = x1
     dets[..., 1] = y1
     dets[..., 2] = dets[..., 2].maximum(x1 + 2)

@@ -107,35 +107,76 @@ def test_letterbox_reorg_fused_on_gpu_equals_two_steps_and_oracle(act):
         assert bool((one[:, :, 0] == 3.0).all()) and bool((one[:, :, W2 + 1:] == 3.0).all()) and bool((one[:, :, 1:W2 + 1, 12:] == 0).all())
 
 
+# (detector canvas (H, W), source frames (h, w)) that are not the identity: 720p into 384 x 640 (gain 1/2, pad 12), 360 x 640 into
+# 384 x 640 (gain 1, pad 12)
+LETTERBOXED = [((384, 640), (720, 1280)), ((384, 640), (360, 640))]
+LETTERBOXED_IDS = ["720p_in_384x640", "360x640_in_384x640"]
+
+
+def _frames(seed, n, src, textured=False):
+    """n frame pairs drifting by (2k, k) px: uniform noise, or (textured) the seeded rectangles-and-noise frames of b200track.synth --
+    noise resized by 1/2 averages out to grey and leaves the detector nothing to find"""
+    from b200track.synth import textured_frame
+    rng = np.random.default_rng(seed)
+    if textured:
+        base = np.stack([textured_frame(seed + s, src[0], src[1], n_rect=300) for s in range(2)])
+    else:
+        base = rng.integers(0, 256, (2,) + tuple(src) + (3,), dtype=np.uint8)
+    return [torch.from_numpy(np.roll(base, (2 * k, k), axis=(1, 2)).copy()).pin_memory() for k in range(n)]
+
+
+def _run(pipe, frames):
+    from b200track import _lib as L
+    got = []
+    for f in frames:
+        r = pipe.step(f)
+        if r is not None:
+            got.append([r[0][s, :int(r[1][s, L.STAT_NOUT])].clone() for s in range(2)])
+    r = pipe.flush()
+    got.append([r[0][s, :int(r[1][s, L.STAT_NOUT])].clone() for s in range(2)])
+    return got
+
+
 def test_pipeline_uint8_frames_equal_float_frames():
     """TrackingPipeline fed uint8 BGR frames (device-side letterbox + ReOrg, 3 bytes per pixel over PCIe) returns the same track
-    rows, frame by frame, as the pipeline fed the float tensors the reference's dataloader would produce from those frames."""
+    rows, frame by frame, as the pipeline fed the float tensors the reference's dataloader would produce from those frames; both
+    declare the source size, so both scale their detections back to the source frame -- and the detections of the last frame
+    are the reference's: letterbox -> detect -> scale_coords(...).round() (tracker/track.py:143-145, 239-240)."""
+    _uint8_equal_float((256, 256), (256, 256))
+
+
+@pytest.mark.parametrize("geo", LETTERBOXED, ids=LETTERBOXED_IDS)
+def test_pipeline_uint8_frames_equal_float_frames_letterboxed(geo):
+    """the same at a source size that is not the canvas: rows in source-frame pixels, clipped to the source frame"""
+    _uint8_equal_float(*geo)
+
+
+def _uint8_equal_float(canvas, src):
     from b200track import _lib as L
     from b200track.detector import DetectorW6
     from b200track.engine import TrackEngine
     from b200track.pipeline import TrackingPipeline
+    from b200track.preprocess import Letterbox
     from b200track.w6 import calibrated_state_dict
+    from utils.general import scale_coords
     sd = calibrated_state_dict(0, 256, "cuda")
-    rng = np.random.default_rng(33)
-    base = rng.integers(0, 256, (2, 256, 256, 3), dtype=np.uint8)
-    frames_u8 = [torch.from_numpy(np.roll(base, (2 * k, k), axis=(1, 2)).copy()).pin_memory() for k in range(5)]
-    frames_f = [(f.flip(-1).permute(0, 3, 1, 2).float() / 255.0).contiguous().pin_memory() for f in frames_u8]   # BGR->RGB, CHW, /255 (:80-86)
-    results = []
+    identity = canvas == src
+    frames_u8 = _frames(33, 5, src, textured=not identity)
+    lb = Letterbox(max(canvas), 64)
+    frames_f = [lb(f.cuda())[0].cpu().pin_memory() for f in frames_u8]          # BGR->RGB, CHW, /255 of the letterboxed frame
+    if canvas == src:
+        assert all(torch.equal(a, (f.flip(-1).permute(0, 3, 1, 2).float() / 255.0)) for a, f in zip(frames_f, frames_u8))
+    results, last = [], []
     for frames in (frames_u8, frames_f):
-        det = DetectorW6(sd, batch=2, img_size=256, use_graph=False, autotune=False)
-        if frames is frames_u8:
-            geo = det.set_source_frames((256, 256))
-            assert (geo["top"], geo["left"], geo["unpad_w"]) == (0, 0, 256)
-        eng = TrackEngine("bytetrack", n_seq=2, cap=512, dmax=300)
+        det = DetectorW6(sd, batch=2, img_size=canvas, use_graph=False, autotune=False)
+        geo_lb = det.set_source_frames(src)
+        if canvas == src:
+            assert (geo_lb["top"], geo_lb["left"], geo_lb["unpad_w"]) == (0, 0, 256)
+        eng = TrackEngine("bytetrack", n_seq=2, cap=512, dmax=300, **({} if identity else dict(conf_thresh=0.1)))
         pipe = TrackingPipeline(det, eng, out_rows=512)
-        got = []
-        for f in frames:
-            r = pipe.step(f)
-            if r is not None:
-                got.append([r[0][s, :int(r[1][s, L.STAT_NOUT])].clone() for s in range(2)])
-        r = pipe.flush()
-        got.append([r[0][s, :int(r[1][s, L.STAT_NOUT])].clone() for s in range(2)])
-        results.append(got)
+        results.append(_run(pipe, frames))
+        torch.cuda.synchronize()
+        last.append((det.out.clone(), det.out_count.clone()))
     assert len(results[0]) == len(results[1]) == 5
     n_rows = 0
     for a, b in zip(*results):
@@ -144,38 +185,72 @@ def test_pipeline_uint8_frames_equal_float_frames():
             assert a[s].shape == b[s].shape and torch.allclose(a[s], b[s], rtol=0, atol=0, equal_nan=True)
             n_rows += a[s].shape[0]
     assert n_rows > 0
+    # the last frame's detections, the reference's way, on a separate detector
+    ref_det = DetectorW6(sd, batch=2, img_size=canvas, use_graph=False, autotune=False)
+    out, cnt = ref_det.detect(lb(frames_u8[-1].cuda())[0], post=False)
+    assert int(cnt.sum()) > 0
+    for (got, gcnt) in last:
+        assert torch.equal(gcnt, cnt)
+        for s in range(2):
+            n = int(cnt[s])
+            exp = out[s, :n].clone()
+            exp[:, :4] = scale_coords(canvas, exp[:, :4], src).round()
+            assert torch.equal(got[s, :n], exp), "sequence %d: rows are not in source-frame pixels" % s
+        assert float(got[:, :, [0, 2]].max()) <= src[1] and float(got[:, :, [1, 3]].max()) <= src[0]
     with pytest.raises(L.B2TError):                                              # mismatched engine layout is refused up front
         TrackingPipeline(det, TrackEngine("bytetrack", n_seq=2, cap=512, dmax=256), out_rows=512)
 
 
-def test_pipeline_twin_detectors_equal_single_detector():
-    """TrackingPipeline over two twin detectors (frames alternate; ingest / NMS / association of neighbouring frames overlap the
-    forward) returns, frame by frame, exactly the rows of the single-detector pipeline."""
+def test_pipeline_refuses_detector_whose_source_geometry_changed():
+    """the pipeline captures the NMS graph with the detector's scale_coords geometry: declaring other source frames afterwards
+    is refused at the next step instead of scaling with the stale one"""
     from b200track import _lib as L
     from b200track.detector import DetectorW6
     from b200track.engine import TrackEngine
     from b200track.pipeline import TrackingPipeline
     from b200track.w6 import calibrated_state_dict
     sd = calibrated_state_dict(0, 256, "cuda")
-    rng = np.random.default_rng(34)
-    base = rng.integers(0, 256, (2, 256, 256, 3), dtype=np.uint8)
-    frames = [torch.from_numpy(np.roll(base, (2 * k, k), axis=(1, 2)).copy()).pin_memory() for k in range(7)]
+    det = DetectorW6(sd, batch=2, img_size=(384, 640), use_graph=False, autotune=False)
+    det.set_source_frames((720, 1280))
+    pipe = TrackingPipeline(det, TrackEngine("bytetrack", n_seq=2, cap=512, dmax=300), out_rows=512)
+    pipe.step(_frames(1, 1, (720, 1280))[0])
+    det.set_source_frames((360, 640))
+    with pytest.raises(L.B2TError, match="geometry changed"):
+        pipe.step(_frames(1, 1, (360, 640))[0])
+    det.set_source_frames((720, 1280))                                          # back to the captured geometry: accepted again
+    pipe.step(_frames(2, 1, (720, 1280))[0])
+    pipe.flush()
+
+
+def test_pipeline_twin_detectors_equal_single_detector():
+    """TrackingPipeline over two twin detectors (frames alternate; ingest / NMS / association of neighbouring frames overlap the
+    forward) returns, frame by frame, exactly the rows of the single-detector pipeline."""
+    _twins_equal_single((256, 256), (256, 256))
+
+
+@pytest.mark.parametrize("geo", LETTERBOXED, ids=LETTERBOXED_IDS)
+def test_pipeline_twin_detectors_equal_single_detector_letterboxed(geo):
+    _twins_equal_single(*geo)
+
+
+def _twins_equal_single(canvas, src):
+    from b200track.detector import DetectorW6
+    from b200track.engine import TrackEngine
+    from b200track.pipeline import TrackingPipeline
+    from b200track.w6 import calibrated_state_dict
+    sd = calibrated_state_dict(0, 256, "cuda")
+    identity = canvas == src
+    frames = _frames(34, 7, src, textured=not identity)
     results = []
     for n_det in (1, 2):
         dets = []
         for _ in range(n_det):
-            d = DetectorW6(sd, batch=2, img_size=256, use_graph=False, autotune=False)
-            d.set_source_frames((256, 256))
+            d = DetectorW6(sd, batch=2, img_size=canvas, use_graph=False, autotune=False)
+            d.set_source_frames(src)
             dets.append(d)
-        pipe = TrackingPipeline(dets if n_det == 2 else dets[0], TrackEngine("bytetrack", n_seq=2, cap=512, dmax=300), out_rows=512)
-        got = []
-        for f in frames:
-            r = pipe.step(f)
-            if r is not None:
-                got.append([r[0][s, :int(r[1][s, L.STAT_NOUT])].clone() for s in range(2)])
-        r = pipe.flush()
-        got.append([r[0][s, :int(r[1][s, L.STAT_NOUT])].clone() for s in range(2)])
-        results.append(got)
+        eng = TrackEngine("bytetrack", n_seq=2, cap=512, dmax=300, **({} if identity else dict(conf_thresh=0.1)))
+        pipe = TrackingPipeline(dets if n_det == 2 else dets[0], eng, out_rows=512)
+        results.append(_run(pipe, frames))
     assert len(results[0]) == len(results[1]) == 7
     rows = 0
     for a, b in zip(*results):

@@ -178,37 +178,52 @@ def test_segmented_extractor_refuses_bad_boxes(extractors):
 
 # ---------------------------------------------------------------- 4 / 5. TrackingPipeline(reid=)
 
-def _scenario(S=3, n=6, size=256):
+# (detector canvas (H, W), source frames (h, w)) that are not the identity: 720p into 384 x 640 (gain 1/2, pad 12) and 360 x 640 into
+# 384 x 640 (gain 1, pad 12) -- pipeline rows are in source-frame pixels, as tracker/track.py:240 produces them
+LETTERBOXED = [((384, 640), (720, 1280)), ((384, 640), (360, 640))]
+LETTERBOXED_IDS = ["720p_in_384x640", "360x640_in_384x640"]
+
+
+def _scenario(S=3, n=6, hw=(256, 256)):
     from b200track.synth import textured_frame
-    base = np.stack([textured_frame(300 + s, size, size, n_rect=300) for s in range(S)])
+    base = np.stack([textured_frame(300 + s, hw[0], hw[1], n_rect=300) for s in range(S)])
     return [torch.from_numpy(np.ascontiguousarray(np.roll(base, (3 * k, -2 * k), axis=(1, 2)))).pin_memory() for k in range(n)]
 
 
-def _detector(sd, S, size=256):
+def _detector(sd, S, canvas=(256, 256), src=(256, 256)):
     from b200track.detector import DetectorW6
-    det = DetectorW6(sd, batch=S, img_size=size, use_graph=False, autotune=False)
-    det.set_source_frames((size, size))
+    det = DetectorW6(sd, batch=S, img_size=canvas, use_graph=False, autotune=False)
+    det.set_source_frames(src)
     return det
 
 
-def _detect(det, f):
+def _reference_rows(det, f):
+    """the reference's way (tracker/track.py:143-145, 239-240): letterbox the frames, detect on the canvas without
+    post-processing, then scale_coords(...).round() back to the source frame with the drop-in utils.general.  Also leaves the
+    frames in det.src_u8.  Returns (rows (S, dmax, 6) float32, counts (S,) int32) device tensors."""
+    from b200track.preprocess import Letterbox
+    from utils.general import scale_coords
     det.src_u8.copy_(f)
-    det.ingest_u8_launch()
-    for fn, _, _ in det.ops[1:]:                     # ops[0] is the ReOrg of the float tensor, replaced by the uint8 ingest
-        fn()
-    det._nms_launch(True)
+    img, _ = Letterbox(max(det.H, det.W), 64)(det.src_u8)
+    assert tuple(img.shape[2:]) == (det.H, det.W)
+    out, cnt = det.detect(img, post=False)
+    rows = out.clone()
+    for s in range(det.B):
+        rows[s, :, :4] = scale_coords((det.H, det.W), rows[s, :, :4], det.src_hw).round()
+    return rows, cnt.clone()
 
 
-def _pick_thresh(det, frames, size=256):
+def _pick_thresh(det, frames):
     """conf_thresh 0.2 unless a frame has no det_high row then (the boxes widened as in the runs below, so none is refused)"""
+    h, w = det.src_hw
     for thr in (0.2, 0.1, 0.05):
         ok = True
         for f in frames:
-            _detect(det, f)
-            P.widen_degenerate(det.out, size)
+            rows, cnt = _reference_rows(det, f)
+            P.widen_degenerate(rows, (h, w))
             torch.cuda.synchronize()
-            d, c = det.out.cpu().numpy(), det.out_count.cpu().numpy()
-            st = P.crop_list_ref(d, c, thr, size, size, d.shape[0] * d.shape[1])[3]
+            d, c = rows.cpu().numpy(), cnt.cpu().numpy()
+            st = P.crop_list_ref(d, c, thr, h, w, d.shape[0] * d.shape[1])[3]
             assert not st[:-1].any()
             ok = ok and st[-1] >= 1
         if ok:
@@ -216,8 +231,9 @@ def _pick_thresh(det, frames, size=256):
     pytest.fail("no det_high rows on this stream")
 
 
-def _widened_pipeline(pipe, size=256):
-    """every detector's NMS output widened on the tracker stream before the crop list (and so before GMC and the step)"""
+def _widened_pipeline(pipe, size=(256, 256)):
+    """every detector's NMS output widened inside the source frame on the tracker stream before the crop list (and so before GMC
+    and the step)"""
     cut = pipe.reid_net.cut
 
     def widened_cut(fr, d, cnt, t):
@@ -239,26 +255,27 @@ def _run_pipeline(pipe, frames, S):
 
 
 def _stepwise(det, eng, ext, frames, S, gmc=None):
-    """detect -> NMS -> [GMC] -> per-sequence features_from_frame of the det_high rows -> scatter -> step_device(feats=), one stream"""
+    """letterbox -> detect -> NMS -> scale_coords to the source frame (the reference's way, not the pipeline's NMS graph) -> [GMC on
+    the source frame] -> per-sequence features_from_frame of the det_high rows -> scatter -> step_device(feats=), one stream"""
     thr = np.float32(eng.cfg.conf_thresh)
     out = torch.zeros((S, eng.cap, L.OUT_COLS), dtype=torch.float64, device="cuda")
     stat = torch.zeros((S, L.STAT_WORDS), dtype=torch.int32, device="cuda")
     feats = torch.zeros((S, eng.dmax, 512), dtype=torch.float32, device="cuda")
     exp, dets = [], []
     for f in frames:
-        _detect(det, f)
-        P.widen_degenerate(det.out, 256)
+        rows, rcnt = _reference_rows(det, f)
+        P.widen_degenerate(rows, det.src_hw)
         w = None
         if gmc is not None:
-            w23, _ = gmc.estimate(det.src_u8, det.out, det.out_count, det_thresh=float(eng.cfg.conf_thresh))
+            w23, _ = gmc.estimate(det.src_u8, rows, rcnt, det_thresh=float(eng.cfg.conf_thresh))
             w = w23.view(S, 6)
-        d = det.out.cpu().numpy(); cnt = det.out_count.cpu().numpy()
+        d = rows.cpu().numpy(); cnt = rcnt.cpu().numpy()
         dets.append([d[s, :cnt[s]].copy() for s in range(S)])
         for s in range(S):
             hi = np.nonzero(d[s, :cnt[s], 4] >= thr)[0]
             if len(hi):
                 feats[s, torch.from_numpy(hi).cuda()] = ext.features_from_frame(det.src_u8[s], d[s, hi, :4])
-        eng.step_device(det.out, det.out_count, out, stat, warps=w, feats=feats)
+        eng.step_device(rows, rcnt, out, stat, warps=w, feats=feats)
         torch.cuda.synchronize()
         assert int(stat[:, L.STAT_ERR].max()) == 0
         exp.append([out[s, :int(stat[s, L.STAT_NOUT])].cpu().clone() for s in range(S)])
@@ -289,16 +306,25 @@ def _engine(S, dmax, thr, use_gmc):
 def test_pipeline_reid_equals_stepwise_and_dropin(w6_sd, extractors):
     """one detector, no GMC: pipeline rows == stepwise rows (bitwise), and == the drop-in BoTSORT(use_apperance_model=True) run per
     sequence on the same NMS rows and frames (ids up to a per-sequence offset, boxes within 1e-9)"""
+    _reid_equals_stepwise_and_dropin(w6_sd, extractors, (256, 256), (256, 256))
+
+
+@pytest.mark.parametrize("geo", LETTERBOXED, ids=LETTERBOXED_IDS)
+def test_pipeline_reid_equals_stepwise_and_dropin_letterboxed(w6_sd, extractors, geo):
+    _reid_equals_stepwise_and_dropin(w6_sd, extractors, *geo)
+
+
+def _reid_equals_stepwise_and_dropin(w6_sd, extractors, canvas, src):
     from b200track.pipeline import TrackingPipeline
     S = 3
-    frames = _scenario(S)
+    frames = _scenario(S, hw=src)
     ext = extractors[("float16", "batch")]
-    det = _detector(w6_sd, S)
+    det = _detector(w6_sd, S, canvas, src)
     thr = _pick_thresh(det, frames)
-    pipe = _widened_pipeline(TrackingPipeline(det, _engine(S, det.max_det, thr, False), out_rows=1152, reid=ext))
+    pipe = _widened_pipeline(TrackingPipeline(det, _engine(S, det.max_det, thr, False), out_rows=1152, reid=ext), src)
     got = _run_pipeline(pipe, frames, S)
     assert int(pipe.h_rstat[0][S]) + int(pipe.h_rstat[1][S]) > 0, "no det_high crops: the test shows nothing"
-    exp, dets = _stepwise(_detector(w6_sd, S), _engine(S, det.max_det, thr, False), ext, frames, S)
+    exp, dets = _stepwise(_detector(w6_sd, S, canvas, src), _engine(S, det.max_det, thr, False), ext, frames, S)
     _assert_rows_equal(got, exp, S)
     # ---- the drop-in, one tracker per sequence (reference tracker/track.py:123,132), fed the same NMS rows and frames
     saved = {k: sys.modules.pop(k) for k in list(sys.modules) if k in ("basetrack", "botsort", "matching", "kalman_filter")}
@@ -339,19 +365,29 @@ def test_pipeline_reid_equals_stepwise_and_dropin(w6_sd, extractors):
 
 
 def test_pipeline_reid_twins_with_gpu_gmc_equals_stepwise(w6_sd, extractors):
+    _reid_twins_with_gmc(w6_sd, extractors, (256, 256), (256, 256))
+
+
+@pytest.mark.parametrize("geo", LETTERBOXED, ids=LETTERBOXED_IDS)
+def test_pipeline_reid_twins_with_gpu_gmc_equals_stepwise_letterboxed(w6_sd, extractors, geo):
+    """twin detectors with GMC on the source frame, at a source size that is not the canvas"""
+    _reid_twins_with_gmc(w6_sd, extractors, *geo)
+
+
+def _reid_twins_with_gmc(w6_sd, extractors, canvas, src):
     from b200track.gmc import GmcEstimator
     from b200track.pipeline import TrackingPipeline
     S = 2
-    frames = _scenario(S)
+    frames = _scenario(S, hw=src)
     ext = extractors[("bfloat16", "batch")]
-    dets = [_detector(w6_sd, S), _detector(w6_sd, S)]
+    dets = [_detector(w6_sd, S, canvas, src), _detector(w6_sd, S, canvas, src)]
     thr = _pick_thresh(dets[0], frames)
-    gmc = GmcEstimator(S, 256, 256, 2, max_kp=4096)
-    pipe = _widened_pipeline(TrackingPipeline(dets, _engine(S, dets[0].max_det, thr, True), out_rows=1152, gmc=gmc, reid=ext))
+    gmc = GmcEstimator(S, src[0], src[1], 2, max_kp=4096)
+    pipe = _widened_pipeline(TrackingPipeline(dets, _engine(S, dets[0].max_det, thr, True), out_rows=1152, gmc=gmc, reid=ext), src)
     got = _run_pipeline(pipe, frames, S)
     warps_pipe = gmc.warps.cpu().numpy().copy()
-    gmc2 = GmcEstimator(S, 256, 256, 2, max_kp=4096)
-    exp, _ = _stepwise(_detector(w6_sd, S), _engine(S, dets[0].max_det, thr, True), ext, frames, S, gmc=gmc2)
+    gmc2 = GmcEstimator(S, src[0], src[1], 2, max_kp=4096)
+    exp, _ = _stepwise(_detector(w6_sd, S, canvas, src), _engine(S, dets[0].max_det, thr, True), ext, frames, S, gmc=gmc2)
     _assert_rows_equal(got, exp, S)
     np.testing.assert_array_equal(warps_pipe, gmc2.warps.cpu().numpy())
 

@@ -10,18 +10,20 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.join(os.path.dirname(__file__), "hostsim"))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import nms_ref as R  # noqa: E402
 from simlib import ptr, sim  # noqa: E402
 from b200track import _lib as L  # noqa: E402
 from oracle import detector as OD  # noqa: E402
 
 
-def _run_nms(pred, conf=0.01, iou=0.45, max_det=300, max_nms=30000, post=0, img=(640.0, 640.0), max_cand=None):
+def _run_nms(pred, conf=0.01, iou=0.45, max_det=300, max_nms=30000, post=0, img=(640.0, 640.0), max_cand=None, geo=(1.0, 0.0, 0.0)):
     lib = sim()
     B, N, no = pred.shape
     max_cand = max_cand or N
     ws = np.zeros(lib.b2t_nms_workspace_bytes(B, max_cand, max_nms), dtype=np.uint8)
     out = np.zeros((B, max_det, 6), dtype=np.float32); cnt = np.zeros(B, dtype=np.int32)
-    rc = lib.b2t_nms(ptr(pred), B, N, no, conf, iou, max_det, max_nms, max_cand, post, 1.0, 0.0, 0.0, img[0], img[1], ptr(ws), ws.size, ptr(out),
+    rc = lib.b2t_nms(ptr(pred), B, N, no, conf, iou, max_det, max_nms, max_cand, post, *geo, img[0], img[1], ptr(ws), ws.size, ptr(out),
                      ptr(cnt), None)
     assert rc == 0, lib.b2t_detect_last_error()
     return out, cnt
@@ -155,3 +157,59 @@ def test_nms_argument_errors():
     assert lib.b2t_nms(ptr(p), 1, 4, 8, -0.5, 0.45, 4, 4, 4, 0, 1.0, 0.0, 0.0, 1.0, 1.0, ptr(ws), ws.size, ptr(out), ptr(cnt), None) != 0
     assert lib.b2t_nms(ptr(p), 1, 4, 8, 0.1, 0.45, 4, 4, 4, 0, 1.0, 0.0, 0.0, 1.0, 1.0, ptr(ws), 16, ptr(out), ptr(cnt), None) != 0
     assert b"workspace" in lib.b2t_detect_last_error()
+    # fewer candidate slots than rows: refused (the surplus would be dropped in whatever order the atomics ran)
+    assert lib.b2t_nms(ptr(p), 1, 4, 8, 0.1, 0.45, 4, 3, 3, 0, 1.0, 0.0, 0.0, 1.0, 1.0, ptr(ws), ws.size, ptr(out), ptr(cnt), None) == -1
+    assert b"max_cand" in lib.b2t_detect_last_error()
+    assert lib.b2t_nms(ptr(p), 1, 4, 8, 0.1, 0.45, 4, 4, 4, 1, 0.0, 0.0, 0.0, 1.0, 1.0, ptr(ws), ws.size, ptr(out), ptr(cnt), None) == -1
+
+
+# ---------------------------------------------------------------- the edge cases of tests/nms_ref.py, bit for bit
+
+def _check_bits(out, cnt, ref):
+    for b, r in enumerate(ref):
+        n = int(cnt[b])
+        assert R.first_row_mismatch(out[b, :n], r["rows"]) is None, "image %d: first differing row %s (%d rows, expected %d)" % (
+            b, R.first_row_mismatch(out[b, :n], r["rows"]), n, len(r["rows"]))
+
+
+@pytest.mark.parametrize("name", sorted(R.edge_cases(large=False)))
+def test_nms_edge_cases_bit_equal_nms_ref(name):
+    pred, conf, iou, max_det, max_nms = R.edge_cases(large=False)[name]
+    out, cnt = _run_nms(np.ascontiguousarray(pred), conf=conf, iou=iou, max_det=max_det, max_nms=max_nms)
+    _check_bits(out, cnt, R.nms_ref(pred, conf, iou, max_det, max_nms))
+
+
+@pytest.mark.parametrize("conf", [0.0, 0.25, 0.999])
+@pytest.mark.parametrize("iou", [0.0, 0.45, 1.0])
+@pytest.mark.parametrize("max_det", [1, 63, 64, 65, 300])
+def test_nms_batch_of_edge_sizes_bit_equal_nms_ref(max_det, iou, conf):
+    """B = 8 images of 0, 1, 63, 64, 65, 700, 64 and 1 candidates (block edges of the 64-row greedy scan)"""
+    pred = R.batch_pred(sizes=(0, 1, 63, 64, 65, 700, 64, 1), N=900, nc=3)
+    out, cnt = _run_nms(pred, conf=conf, iou=iou, max_det=max_det)
+    _check_bits(out, cnt, R.nms_ref(pred, conf, iou, max_det, 30000))
+
+
+@pytest.mark.parametrize("k", range(len(R.GEOMETRIES)))
+def test_nms_post_geometry_in_band_and_reciprocal_form(k):
+    """post = 1 with the scale_coords geometry of a letterboxed source: every coordinate inside the float64 band of
+    tests/nms_ref.py, and equal to ``(x - pad) * (1 / gain)`` in fp32, clipped and rounded half to even"""
+    src, canvas = R.GEOMETRIES[k]
+    rows = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "scale_coords.npz"))["rows%d" % k]
+    n = len(rows)
+    pred = np.zeros((1, n, 6), np.float32)
+    pred[0, :, 0] = (rows[:, 0] + rows[:, 2]) / 2; pred[0, :, 2] = rows[:, 2] - rows[:, 0]
+    pred[0, :, 1] = (rows[:, 1] + rows[:, 3]) / 2; pred[0, :, 3] = rows[:, 3] - rows[:, 1]
+    pred[0, :, 4] = np.linspace(0.99, 0.5, n, dtype=np.float32)
+    pred[0, :, 5] = 1.0
+    gain, pw, ph = R.scale_geometry(canvas, src)
+    post0, cnt0 = _run_nms(pred, iou=1.0, max_det=300)
+    post1, cnt1 = _run_nms(pred, iou=1.0, max_det=300, post=1, img=(float(src[1]), float(src[0])), geo=(gain, pw, ph))
+    m = int(cnt0[0])
+    assert m == int(cnt1[0]) == n
+    got, base = post1[0, :m], post0[0, :m]
+    lo, hi, _ = R.scale_coords_ref(base, canvas, src)
+    assert len(R.outside_band(got, lo, hi)) == 0
+    pad = np.array([pw, ph, pw, ph], np.float32)
+    rec = np.round(np.clip(((base[:, :4] - pad) * (np.float32(1) / np.float32(gain))).astype(np.float32), 0,
+                           np.array([src[1], src[0]] * 2, np.float32)))
+    assert np.array_equal(got[:, :4], rec) and np.array_equal(got[:, 4:], base[:, 4:])

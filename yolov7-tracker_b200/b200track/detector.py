@@ -245,6 +245,9 @@ class DetectorW6:
         self.max_cand = self.n_total
         ws = lib.b2t_nms_workspace_bytes(batch, self.max_cand, max_nms)
         self.nms_ws = torch.empty(ws, dtype=torch.uint8, device=self.dev)
+        # post-processing geometry of the NMS output (gain, pad_w, pad_h, clip width, clip height): the identity on the canvas until
+        # set_source_frames declares the frames' size, then scale_coords back to the source frame (tracker/track.py:240)
+        self.post_geo = (1.0, 0.0, 0.0, float(W), float(H))
         self.graph, self.graph_post = None, None
         self.fwd_graph = None
         self.use_graph = use_graph
@@ -301,10 +304,11 @@ class DetectorW6:
             fn()
 
     def _nms_launch(self, post=True):
-        """Detect decode fused with NMS, straight from the four raw head maps (b2t_detect_nms): `pred` is not touched."""
+        """Detect decode fused with NMS, straight from the four raw head maps (b2t_detect_nms): `pred` is not touched.  post: rows
+        scaled to the source frame declared by set_source_frames (the canvas when none was), clipped and rounded."""
         lib = self.lib
         rc = lib.b2t_detect_nms(C.cast(self.head_levels, C.c_void_p), len(self.head_levels), self.B, NO, self.conf_thres, self.iou_thres,
-                                self.max_det, self.max_nms, self.max_cand, int(post), 1.0, 0.0, 0.0, float(self.W), float(self.H),
+                                self.max_det, self.max_nms, self.max_cand, int(post), *self.post_geo,
                                 C.c_void_p(self.nms_ws.data_ptr()), self.nms_ws.numel(), C.c_void_p(self.out.data_ptr()),
                                 C.c_void_p(self.out_count.data_ptr()), C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream))
         _check(lib, rc, "detect_nms")
@@ -313,7 +317,7 @@ class DetectorW6:
         """non_max_suppression on the materialised `pred` tensor (b2t_nms) -- the two-step path decode() + NMS."""
         lib = self.lib
         rc = lib.b2t_nms(C.c_void_p(self.pred.data_ptr()), self.B, self.n_total, NO, self.conf_thres, self.iou_thres, self.max_det, self.max_nms,
-                         self.max_cand, int(post), 1.0, 0.0, 0.0, float(self.W), float(self.H), C.c_void_p(self.nms_ws.data_ptr()),
+                         self.max_cand, int(post), *self.post_geo, C.c_void_p(self.nms_ws.data_ptr()),
                          self.nms_ws.numel(), C.c_void_p(self.out.data_ptr()), C.c_void_p(self.out_count.data_ptr()),
                          C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream))
         _check(lib, rc, "nms")
@@ -328,8 +332,10 @@ class DetectorW6:
     def set_source_frames(self, src_hw):
         """uint8 ingest: declare the (height, width) of the raw BGR frames this detector will be fed.  Allocates the device
         staging buffer ``self.src_u8`` (B, h, w, 3) and checks that the reference's letterbox geometry
-        (tracker/tracker_dataloader.py:100-126, stride 64 minimum rectangle) produces exactly this detector's (H, W)."""
-        from .preprocess import letterbox_geometry
+        (tracker/tracker_dataloader.py:100-126, stride 64 minimum rectangle) produces exactly this detector's (H, W).
+        From then on post-processed NMS rows (``detect(post=True)``, ``nms_from_pred(True)``, the pipeline) are in source-frame
+        pixels: scale_coords from the canvas to (h, w), clipped to the frame, rounded (tracker/track.py:240)."""
+        from .preprocess import letterbox_geometry, scale_coords_geometry
         if not self.stem_padded:
             raise L.B2TError("the uint8 ingest writes the ReOrg layout of the w6 stem: this graph takes the float tensor")
         h, w = int(src_hw[0]), int(src_hw[1])
@@ -337,6 +343,10 @@ class DetectorW6:
         if (geo["out_h"], geo["out_w"]) != (self.H, self.W):
             raise L.B2TError("frames of %dx%d letterbox to %dx%d, this detector was planned for %dx%d" % (h, w, geo["out_h"], geo["out_w"], self.H, self.W))
         self.src_geo, self.src_hw = geo, (h, w)
+        post_geo = scale_coords_geometry((self.H, self.W), (h, w)) + (float(w), float(h))
+        if post_geo != self.post_geo:
+            self.graph = None                                                  # the captured NMS epilogue scales differently: capture again
+        self.post_geo = post_geo
         self.src_u8 = torch.zeros((self.B, h, w, 3), dtype=torch.uint8, device=self.dev)
         return geo
 

@@ -76,6 +76,7 @@ class TrackingPipeline:
         self.ev_out_free = ev()      # the tracker step has consumed det.out
         self.ev_trk_done = [torch.cuda.Event(), torch.cuda.Event()]
         self.g_fwd, self.g_nms = [None] * nd, [None] * nd
+        self.post_geo = [d.post_geo for d in self.dets]                     # the scale_coords geometry each NMS graph was captured with
         self.n = 0
         self._capture()
 
@@ -114,6 +115,9 @@ class TrackingPipeline:
             raise L.B2TError("TrackingPipeline(reid=): frames must be uint8 BGR (the crops are cut from det.src_u8), got %s" % frames.dtype)
         if u8 and (getattr(det, "src_u8", None) is None or tuple(frames.shape) != tuple(det.src_u8.shape)):
             raise L.B2TError("uint8 frames of shape %s: call det.set_source_frames((h, w)) first" % (tuple(frames.shape),))
+        if det.post_geo != self.post_geo[i]:
+            raise L.B2TError("the detector's source-frame geometry changed after the pipeline captured its NMS graph "
+                             "(call set_source_frames before building the TrackingPipeline)")
         # ---- input: copy once the previous ingest of this detector has read the staging buffer; the ingest kernel follows on the same
         # stream as soon as the detector's previous forward has consumed the stem input (twin mode) / on the detect stream (single)
         s_in = self.s_copy if self.twin else self.s_det

@@ -31,6 +31,15 @@ def letterbox_geometry(shape_hw, new_shape=(1280, 1280), stride=32, auto=True, s
             "out_h": unpad_h + top + bottom, "out_w": unpad_w + left + right, "ratio": (r, r), "pad": (float(dw), float(dh))}
 
 
+def scale_coords_geometry(canvas_hw, src_hw):
+    """(gain, pad_w, pad_h) of ``scale_coords(img1_shape, coords, img0_shape, ratio_pad=None)`` (utils/general.py:319-332), the call
+    tracker/track.py:240 makes to map NMS rows from the (H, W) canvas back to the (h, w) source frame.  Recomputed from the two
+    shapes as the reference does, not taken from the letterbox: for 721 x 1283 -> 768 x 1280 it gives pad_h 24.3429, where the
+    letterbox placed the image at 24.5.  Same-size frames give (1.0, 0.0, 0.0)."""
+    gain = min(canvas_hw[0] / src_hw[0], canvas_hw[1] / src_hw[1])
+    return gain, (canvas_hw[1] - src_hw[1] * gain) / 2, (canvas_hw[0] - src_hw[0] * gain) / 2
+
+
 def launch_letterbox(lib, src_ptr, batch, h, w, pitch, geo, out_ptr, stream_ptr, pad_value=114):
     """One call of the C ABI entry point on raw pointers (also how tests/hostsim drives the simulator build)."""
     rc = lib.b2t_letterbox(C.c_void_p(src_ptr), batch, h, w, pitch, geo["unpad_w"], geo["unpad_h"], geo["top"], geo["left"], geo["out_h"], geo["out_w"],

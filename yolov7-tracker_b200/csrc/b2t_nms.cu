@@ -185,18 +185,22 @@ __global__ void bucket_rank_kernel(const Cand* __restrict__ cand, const BKey* __
     sorted[(long long)b * max_nms + r] = cd;
 }
 
-B2T_DEV bool iou_gt(const float4 a, const float4 b, float thr) {     // torchvision nms_kernel devIoU
+// torchvision nms_kernel devIoU, every operation rounded on its own: the unit is built with FMA contraction (the fused decode
+// shares b2t_decode.cuh with b2t_detect.cu and must keep its floats), so the _rn intrinsics stop nvcc from fusing the union's
+// sa + sb - inter or the areas into FFMAs -- a pair at the threshold then gets the decision the unfused fp32 arithmetic of
+// the oracle and tests/nms_ref.py gives it
+B2T_DEV bool iou_gt(const float4 a, const float4 b, float thr) {
     const float left = fmaxf(a.x, b.x), right = fminf(a.z, b.z);
     const float top = fmaxf(a.y, b.y), bottom = fminf(a.w, b.w);
-    const float w = fmaxf(right - left, 0.f), h = fmaxf(bottom - top, 0.f);
-    const float inter = w * h;
-    const float sa = (a.z - a.x) * (a.w - a.y), sb = (b.z - b.x) * (b.w - b.y);
-    return inter / (sa + sb - inter) > thr;
+    const float w = fmaxf(__fsub_rn(right, left), 0.f), h = fmaxf(__fsub_rn(bottom, top), 0.f);
+    const float inter = __fmul_rn(w, h);
+    const float sa = __fmul_rn(__fsub_rn(a.z, a.x), __fsub_rn(a.w, a.y)), sb = __fmul_rn(__fsub_rn(b.z, b.x), __fsub_rn(b.w, b.y));
+    return __fdiv_rn(inter, __fsub_rn(__fadd_rn(sa, sb), inter)) > thr;
 }
 
 __global__ void __launch_bounds__(kGreedyThreads)
 nms_greedy_kernel(const Cand* __restrict__ sorted, const float4* __restrict__ sbox, const int* __restrict__ count, int maxc, int max_nms,
-                  int max_det, float thr, float* __restrict__ out, int* __restrict__ out_count, int post, float gain, float padw, float padh,
+                  int max_det, float thr, float* __restrict__ out, int* __restrict__ out_count, int post, float inv_gain, float padw, float padh,
                   float img_w, float img_h) {
     B2T_DYN_SMEM(dyn);
     float4* kept = reinterpret_cast<float4*>(dyn);                   // class-offset boxes of the rows kept so far [max_det]
@@ -258,7 +262,10 @@ nms_greedy_kernel(const Cand* __restrict__ sorted, const float4* __restrict__ sb
             const Cand cd = sc[i0 + rq];
             float x1 = cd.x1, y1 = cd.y1, x2 = cd.x2, y2 = cd.y2;
             if (post) {
-                x1 = (x1 - padw) / gain; x2 = (x2 - padw) / gain; y1 = (y1 - padh) / gain; y2 = (y2 - padh) / gain;   // scale_coords
+                // scale_coords (utils/general.py:328-330) as torch runs it on a CUDA tensor: `-= pad` in fp32, and `/= gain` by a Python
+                // scalar as a multiply by the fp32 reciprocal (see sort_and_select)
+                x1 = __fmul_rn(__fsub_rn(x1, padw), inv_gain); x2 = __fmul_rn(__fsub_rn(x2, padw), inv_gain);
+                y1 = __fmul_rn(__fsub_rn(y1, padh), inv_gain); y2 = __fmul_rn(__fsub_rn(y2, padh), inv_gain);
                 x1 = fminf(fmaxf(x1, 0.f), img_w); x2 = fminf(fmaxf(x2, 0.f), img_w);                                  // clip_coords
                 y1 = fminf(fmaxf(y1, 0.f), img_h); y2 = fminf(fmaxf(y2, 0.f), img_h);
                 x1 = rintf(x1); y1 = rintf(y1); x2 = rintf(x2); y2 = rintf(y2);                                       // .round()
@@ -317,8 +324,10 @@ int sort_and_select(const Workspace& ws, int B, float iou_thres, int max_det, in
     B2T_LAUNCH(bucket_scatter_kernel, dim3((max_cand + 255) / 256, B), 256, 0, s, ws.cand, ws.count, max_cand, ws.base, ws.cursor, ws.keys);
     B2T_LAUNCH(bucket_rank_kernel, dim3((max_cand + 255) / 256, B), 256, 0, s, ws.cand, ws.keys, ws.count, max_cand, ws.base, ws.hist, max_nms,
                4096.f, ws.sbox, ws.sorted);
+    // torch's CUDA true division by a CPU scalar multiplies by opmath(1) / opmath(scalar): 1.0f / (float)gain, rounded once
+    const float inv_gain = 1.0f / gain;
     B2T_LAUNCH(nms_greedy_kernel, B, kGreedyThreads, (size_t)max_det * sizeof(float4), s, ws.sorted, ws.sbox, ws.count, max_cand, max_nms, max_det,
-               iou_thres, out, out_count, post, gain, padw, padh, img_w, img_h);
+               iou_thres, out, out_count, post, inv_gain, padw, padh, img_w, img_h);
     return ncheck("nms");
 }
 
@@ -336,6 +345,9 @@ extern "C" int b2t_nms(const float* pred, int B, int N, int no, float conf_thres
     if (!pred || !workspace || !out || !out_count || B < 1 || N < 1 || no < 6 || max_det < 1 || max_nms < 1 || max_cand < 1)
         return nfail(B2T_EINVAL, "b2t_nms: bad arguments");
     if (max_det > 2048 || !(conf_thres >= 0.f)) return nfail(B2T_EINVAL, "b2t_nms: need max_det <= 2048 and conf_thres >= 0");
+    // every row may pass the filter: fewer slots would drop candidates in whatever order the atomics ran
+    if (max_cand < N) return nfail(B2T_EINVAL, "b2t_nms: max_cand < N (rows per image)");
+    if (!(gain > 0.f)) return nfail(B2T_EINVAL, "b2t_nms: need gain > 0");
     if (max_nms > max_cand) max_nms = max_cand;
     if (workspace_bytes < b2t_nms_workspace_bytes(B, max_cand, max_nms)) return nfail(B2T_EINVAL, "b2t_nms: workspace too small");
     cudaStream_t s = (cudaStream_t)stream;
@@ -353,8 +365,6 @@ extern "C" int b2t_detect_nms(const b2t_head_level* levels, int n_levels, int B,
     if (!levels || n_levels < 1 || n_levels > 4 || !workspace || !out || !out_count || B < 1 || no < 6 || max_det < 1 || max_nms < 1 || max_cand < 1)
         return nfail(B2T_EINVAL, "b2t_detect_nms: bad arguments");
     if (max_det > 2048 || !(conf_thres >= 0.f)) return nfail(B2T_EINVAL, "b2t_detect_nms: need max_det <= 2048 and conf_thres >= 0");
-    if (max_nms > max_cand) max_nms = max_cand;
-    if (workspace_bytes < b2t_nms_workspace_bytes(B, max_cand, max_nms)) return nfail(B2T_EINVAL, "b2t_detect_nms: workspace too small");
     HeadLevels L;
     memset(&L, 0, sizeof(L));
     L.n_levels = n_levels;
@@ -368,6 +378,10 @@ extern "C" int b2t_detect_nms(const b2t_head_level* levels, int n_levels, int B,
         first += (long long)lv.h * lv.w * 3;
     }
     L.per_image = first;
+    if (max_cand < L.per_image) return nfail(B2T_EINVAL, "b2t_detect_nms: max_cand < rows per image (3 h w summed over the levels)");
+    if (!(gain > 0.f)) return nfail(B2T_EINVAL, "b2t_detect_nms: need gain > 0");
+    if (max_nms > max_cand) max_nms = max_cand;
+    if (workspace_bytes < b2t_nms_workspace_bytes(B, max_cand, max_nms)) return nfail(B2T_EINVAL, "b2t_detect_nms: workspace too small");
     cudaStream_t s = (cudaStream_t)stream;
     Workspace ws;
     carve(workspace, B, max_cand, max_nms, &ws);

@@ -13,6 +13,11 @@
     sim::launch(dim3(grid), dim3(block), (size_t)(smem), [&] { kernel(__VA_ARGS__); })
 #define B2T_SET_SMEM(kernel, bytes) 0
 #define B2T_PREFETCH_L1(ptr) ((void)(ptr))
+// single-rounded IEEE fp32 operations: the simulator library is built with -ffp-contract=off, so nothing fuses them
+inline float __fadd_rn(float a, float b) { return a + b; }
+inline float __fsub_rn(float a, float b) { return a - b; }
+inline float __fmul_rn(float a, float b) { return a * b; }
+inline float __fdiv_rn(float a, float b) { return a / b; }
 #else
 #include <cuda_runtime.h>
 #define B2T_DYN_SMEM(name) extern __shared__ __align__(1024) unsigned char name[]
