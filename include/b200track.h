@@ -306,6 +306,33 @@ int b2t_gmc_estimate_prepared(int n_seq, int height, int width, int downscale, c
  * key points [2][max_kp] (x | y << 16), descriptors [2][max_kp][8 words], working height, working width, matched points */
 int b2t_gmc_workspace_layout(int n_seq, int height, int width, int downscale, int max_kp, size_t* out, int n);
 
+/* ---------------------------------------------------------------- ECC camera-motion estimation (csrc/b2t_ecc.cu)
+ * GMC.applyEcc, method 'ecc' (tracker/botsort.py:78-109; built by StrongSORT.__init__ with downscale 2), for n_seq sequences at once:
+ * BGR2GRAY, for downscale > 1 GaussianBlur((3, 3), 1.5) and resize to (w / ds, h / ds) (:81-90); a sequence's FIRST frame becomes its
+ * template and is never replaced (quirk q17: every later frame is aligned to frame 1); then cv2.findTransformECC(MOTION_EUCLIDEAN,
+ * max_iter iterations, eps) of the frame against the template.  warps_out[n_seq][6]: the 2 x 3 map in row-major order, float32
+ * values in doubles, in DOWN-SCALED pixels (the reference does not scale it back); identity on the first frame; after a failure
+ * (NaN rho, lambda_d <= 0) the map after the last completed update.  stat: [n_seq][B2T_GMC_STAT_WORDS] ints or NULL: iterations
+ * run, the final rho as the low / high words of a double, 0, 0, flags (B2T_ECC_*), 0, frame index.  frames_bgr: [n_seq][height]
+ * [pitch bytes] uint8 BGR in device memory.  The workspace (b2t_ecc_workspace_bytes, caller-owned, zeroed once by b2t_ecc_reset,
+ * which starts new templates) holds each sequence's template and current plane.  Geometry below 8 x 8 working pixels, max_iter
+ * outside [1, 100000] or eps < 0 return B2T_EINVAL.  Never allocates, never synchronises; everything is enqueued on `stream`. */
+#define B2T_ECC_FIRST_FRAME 1
+#define B2T_ECC_CONVERGED 2
+#define B2T_ECC_ITER_CAP 4
+#define B2T_ECC_FAILED_NAN 8
+#define B2T_ECC_FAILED_LAMBDA 16
+size_t b2t_ecc_workspace_bytes(int n_seq, int height, int width, int downscale);
+int b2t_ecc_reset(void* workspace, int n_seq, int height, int width, int downscale, void* stream);
+int b2t_ecc_estimate(const unsigned char* frames_bgr, int n_seq, int height, int width, int pitch, int downscale, int max_iter, double eps,
+                     void* workspace, double* warps_out, int* stat, void* stream);
+/* tests / tools: out[0..5] = slice stride, state, template plane, current plane, working height, working width (byte offsets) */
+int b2t_ecc_workspace_layout(int n_seq, int height, int width, int downscale, size_t* out, int n);
+/* tests: the warp stage of one ECC iteration for a whole (height, width) uint8 plane under map_host[6] (float32, on the HOST):
+ * warpAffine(INTER_LINEAR | WARP_INVERSE_MAP) of the plane and of its two gradients, and the warped all-ones mask (INTER_NEAREST). */
+int b2t_ecc_warp(const unsigned char* plane, int height, int width, const float* map_host, float* img, float* gx, float* gy, unsigned char* mask,
+                 void* stream);
+
 /* ---------------------------------------------------------------- appearance branch glue (csrc/b2t_reid.cu, SURVEY 8f row 3)
  * The reference's ReID extractor (tracker/reid_models/deepsort_reid.py:63-153: a ResNet-style net on 64 x 128 crops -> 512-d unit
  * vectors) runs as plans of the conv kernel above -- BatchNorm folded, act = 2 for ReLU -- plus these element-wise kernels; the cosine GEMM

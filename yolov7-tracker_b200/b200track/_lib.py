@@ -19,6 +19,7 @@ REID_OVERFLOW, REID_ZERO_SIZE, REID_NEGATIVE = 1, 2, 4       # b2t_reid_crops_fr
 OUT_COLS, STAT_WORDS, STAT_PHASE0, STAT_SUB0 = 8, 64, 16, 32
 STAT_NAPP, STAT_NAPPLOW = 30, 31          # appearance pairs, and those whose cost the appearance lowered
 GMC_STAT_WORDS, GMC_FIRST_FRAME, GMC_FEW_POINTS, GMC_TRUNCATED = 8, 1, 2, 4
+ECC_FIRST_FRAME, ECC_CONVERGED, ECC_ITER_CAP, ECC_FAILED_NAN, ECC_FAILED_LAMBDA = 1, 2, 4, 8, 16      # stat word 5 of b2t_ecc_estimate
 (STAT_NOUT, STAT_NEXT_ID, STAT_NTRACKED, STAT_NLOST, STAT_ERR, STAT_FRAME, STAT_NPOOL, STAT_NBIRTH,
  STAT_NHI, STAT_NLO, STAT_NEDGE, STAT_NMATCH0) = range(12)
 FMT_BY_NAME = {"default": FMT_XYAH, "botsort": FMT_XYWH, "strongsort": FMT_NSA}
@@ -97,6 +98,11 @@ SIGNATURES = {
     "b2t_gmc_prepare": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _I, _P]),
     "b2t_gmc_estimate_prepared": (_I, [_I, _I, _I, _I, _P, _P, _I, C.c_float, _P, _I, _I, _P, _P, _P]),
     "b2t_gmc_workspace_layout": (_I, [_I, _I, _I, _I, _I, C.POINTER(_SZ), _I]),
+    "b2t_ecc_workspace_bytes": (_SZ, [_I, _I, _I, _I]),
+    "b2t_ecc_reset": (_I, [_P, _I, _I, _I, _I, _P]),
+    "b2t_ecc_estimate": (_I, [_P, _I, _I, _I, _I, _I, _I, _D, _P, _P, _P, _P]),
+    "b2t_ecc_workspace_layout": (_I, [_I, _I, _I, _I, C.POINTER(_SZ), _I]),
+    "b2t_ecc_warp": (_I, [_P, _I, _I, C.POINTER(C.c_float), _P, _P, _P, _P, _P]),
     "b2t_reid_crops": (_I, [_P, _P, _I, _P, _I, _P]),
     "b2t_maxpool3x3s2": (_I, [_P, _P, _I, _I, _I, _I, _I, _P]),
     "b2t_maxpool2x2s2": (_I, [_P, _P, _I, _I, _I, _I, _I, _P]),
@@ -130,7 +136,7 @@ REID_SYMBOLS = ["b2t_reid_crops", "b2t_maxpool3x3s2", "b2t_maxpool2x2s2", "b2t_a
                 "b2t_avgpool_l2norm_rows"]
 
 # the association branch (csrc/b2t_tracker.cu); the rest are the detector's translation units
-TRACKER_SYMBOLS = [n for n in SIGNATURES if not n.startswith(("b2t_conv", "b2t_detect", "b2t_image", "b2t_upsample", "b2t_spp", "b2t_nms", "b2t_letterbox", "b2t_gmc_workspace", "b2t_gmc_reset", "b2t_gmc_estimate", "b2t_gmc_prepare",
+TRACKER_SYMBOLS = [n for n in SIGNATURES if not n.startswith(("b2t_conv", "b2t_detect", "b2t_image", "b2t_upsample", "b2t_spp", "b2t_nms", "b2t_letterbox", "b2t_gmc_workspace", "b2t_gmc_reset", "b2t_gmc_estimate", "b2t_gmc_prepare", "b2t_ecc",
                                                                    "b2t_reid", "b2t_maxpool", "b2t_add_relu", "b2t_avgpool", "b2t_batchnorm"))]
 
 

@@ -154,6 +154,27 @@ def textured_frame(seed, height=720, width=1280, n_rect=400):
     return np.clip(bgr, 0, 255).astype(np.uint8)
 
 
+def moved_frame(frame, angle_deg=0.0, tx=0.0, ty=0.0):
+    """``frame`` rotated by ``angle_deg`` about its centre, then shifted by (tx, ty) pixels: bilinear, edge pixels repeated.  NumPy
+    only; the source coordinates are floored to 1/256 px and the weights are integers, so every platform builds the same bytes."""
+    h, w = frame.shape[:2]
+    a = np.deg2rad(angle_deg)
+    c, s = np.cos(a), np.sin(a)
+    ys, xs = np.mgrid[0:h, 0:w].astype(np.float64)
+    cx, cy = (w - 1) * 0.5, (h - 1) * 0.5
+    dx, dy = xs - cx - tx, ys - cy - ty
+    U = np.floor((c * dx + s * dy + cx) * 256.0).astype(np.int64)
+    V = np.floor((-s * dx + c * dy + cy) * 256.0).astype(np.int64)
+    fx, fy = U & 255, V & 255
+    x0, y0 = np.clip(U >> 8, 0, w - 1), np.clip(V >> 8, 0, h - 1)
+    x1, y1 = np.clip((U >> 8) + 1, 0, w - 1), np.clip((V >> 8) + 1, 0, h - 1)
+    f = frame.astype(np.int64)
+    fx, fy = fx[..., None], fy[..., None]
+    top = (256 - fx) * f[y0, x0] + fx * f[y0, x1]
+    bot = (256 - fx) * f[y1, x0] + fx * f[y1, x1]
+    return (((256 - fy) * top + fy * bot + (1 << 15)) >> 16).astype(np.uint8)
+
+
 def with_flat_boxes(frame, rng, xywh=False):
     """The frame's detections plus boxes the tracker ignores (zero height, a point, a NaN box; with the xywh Kalman filter also zero width),
     high and low scores, inserted at random places; the frame's own detections keep their order."""

@@ -25,6 +25,7 @@ UNITS = [
     ("b2t_nms.cu", []),
     ("b2t_preproc.cu", ["--fmad=false"]),
     ("b2t_gmc.cu", ["--fmad=false"]),
+    ("b2t_ecc.cu", ["--fmad=false"]),
     ("b2t_reid.cu", []),
 ]
 

@@ -21,6 +21,7 @@
 #include <string>          // before b2t_platform.cuh (the simulator's __noinline__ macro must not reach libstdc++)
 #include <math.h>
 #include "b2t_platform.cuh"
+#include "b2t_luma.cuh"
 #include "../../include/b200track.h"
 
 namespace b2t { void set_detect_error(const char* m); }
@@ -86,21 +87,7 @@ template <class T> B2T_DEV T* wsp(unsigned char* ws, const GmcGeom& g, int seq, 
     return reinterpret_cast<T*>(ws + (size_t)seq * g.stride + off);
 }
 
-// ---------------------------------------------------------------------------------------------- gray + 1/ds scale
-B2T_DEV int gray_of(const unsigned char* q) { return (q[0] * 3735 + q[1] * 19235 + q[2] * 9798 + (1 << 14)) >> 15; }
-
-B2T_DEV void lin_tap(int d, double scale, int src, int& s, int& w0, int& w1, bool clamp_weight) {     // cv2.resize, 8-bit linear (b2t_preproc.cu)
-    float f = (float)((d + 0.5) * scale - 0.5);
-    s = (int)floorf(f);
-    f -= (float)s;
-    if (clamp_weight) {
-        if (s < 0) { f = 0.f; s = 0; }
-        if (s >= src - 1) { f = 0.f; s = src - 1; }
-    }
-    w1 = __float2int_rn(f * 2048.f);
-    w0 = __float2int_rn((1.f - f) * 2048.f);
-}
-
+// ---------------------------------------------------------------------------------------------- gray + 1/ds scale (b2t_luma.cuh)
 __global__ void gray_kernel(const unsigned char* __restrict__ frames, unsigned char* ws, GmcGeom g, double scale_x, double scale_y) {
     const int seq = blockIdx.y;
     const unsigned char* img = frames + (size_t)seq * g.src_h * g.pitch;
@@ -116,18 +103,7 @@ __global__ void gray_kernel(const unsigned char* __restrict__ frames, unsigned c
             const unsigned char* q1 = q0 + g.pitch;
             v = (gray_of(q0) + gray_of(q0 + 3) + gray_of(q1) + gray_of(q1 + 3) + 2) >> 2;
         } else {
-            int sx, a0, a1, sy, b0, b1;
-            lin_tap(x, scale_x, g.src_w, sx, a0, a1, true);
-            lin_tap(y, scale_y, g.src_h, sy, b0, b1, false);
-            const int sx1 = sx + 1 < g.src_w ? sx + 1 : g.src_w - 1;
-            const int y0 = sy < 0 ? 0 : (sy > g.src_h - 1 ? g.src_h - 1 : sy);
-            const int y1 = sy + 1 < 0 ? 0 : (sy + 1 > g.src_h - 1 ? g.src_h - 1 : sy + 1);
-            const unsigned char* r0 = img + (size_t)y0 * g.pitch;
-            const unsigned char* r1 = img + (size_t)y1 * g.pitch;
-            const int h0 = gray_of(r0 + sx * 3) * a0 + gray_of(r0 + sx1 * 3) * a1;
-            const int h1 = gray_of(r1 + sx * 3) * a0 + gray_of(r1 + sx1 * 3) * a1;
-            v = (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
-            v = v < 0 ? 0 : (v > 255 ? 255 : v);
+            v = resize_linear_px([&](int yy, int xx) { return gray_of(img + (size_t)yy * g.pitch + xx * 3); }, x, y, g.src_h, g.src_w, scale_x, scale_y);
         }
         out[i] = (unsigned char)v;
     }

@@ -6,8 +6,9 @@ predict, ``multi_gmc`` of the pool and of the unconfirmed tracks (:380-382), thr
 births from ALL first-stage leftovers (q3), list algebra.  ``multi_gmc`` (:250-269) is also
 available on its own for lists of STrack (b2t_gmc_apply).
 
-Camera-motion ESTIMATION (``GMC.apply``, method 'orb', reference :111-235 -- SURVEY.md section 8(f) row 1)
-runs on the GPU as well (``b200track/gmc.py``, csrc/b2t_gmc.cu).  ``tracker.gmc`` may be replaced by any object
+Camera-motion ESTIMATION (``GMC.apply``, method 'orb', reference :111-235 -- SURVEY.md section 8(f) row 1 -- and
+method 'ecc', reference :78-109, what StrongSORT builds) runs on the GPU as well (``b200track/gmc.py``, csrc/b2t_gmc.cu,
+csrc/b2t_ecc.cu).  ``tracker.gmc`` may be replaced by any object
 with ``apply(raw_frame, detections)`` returning a 2x3 matrix."""
 import numpy as np
 
@@ -22,8 +23,9 @@ import torch  # noqa: E402
 class GMC:
     """``GMC(method='orb', downscale=2)`` -- what ``BoTSORT.__init__`` (reference :286) builds -- runs on the GPU estimator
     (csrc/b2t_gmc.cu through b200track/gmc.py): same key points, descriptors and matches as the reference's OpenCV calls, RANSAC
-    with its own sampling sequence.  'file' and 'none' need no estimation.  'sift' and 'ecc' (unused by BoT-SORT; StrongSORT's
-    ECC is outside SURVEY.md section 8) are not built and raise."""
+    with its own sampling sequence.  ``GMC(method='ecc')`` -- what StrongSORT builds -- runs on ``EccEstimator`` (csrc/b2t_ecc.cu):
+    the same preparation bit for bit and findTransformECC's Euclidean loop, aligned to the FIRST frame as the reference does.
+    'file' and 'none' need no estimation.  'sift' (used by no reference tracker) is not built and raises."""
 
     def __init__(self, method='orb', downscale=2, verbose=None, max_keypoints=32768):
         self.method = method
@@ -31,10 +33,10 @@ class GMC:
         self.max_keypoints = int(max_keypoints)
         self.initializedFirstFrame = False
         self._est = None
-        if method == 'orb':
+        if method in ('orb', 'ecc'):
             pass
-        elif method in ('sift', 'ecc'):
-            raise NotImplementedError("GMC method %r is not built (SURVEY.md section 8f covers the ORB estimator BoT-SORT uses)" % method)
+        elif method == 'sift':
+            raise NotImplementedError("GMC method 'sift' is not built (no reference tracker uses it; 'orb' and 'ecc' run on the GPU)")
         elif method in ('file', 'files'):
             seq, ablation = verbose[0], verbose[1]
             root = 'tracker/GMC_files/MOT17_ablation' if ablation else 'tracker/GMC_files/MOTChallenge'
@@ -50,6 +52,8 @@ class GMC:
     def apply(self, raw_frame, detections=None):
         if self.method == 'orb':
             return self.applyFeaures(raw_frame, detections)
+        if self.method == 'ecc':
+            return self.applyEcc(raw_frame, detections)
         if self.method in ('file', 'files'):
             return self.applyFile(raw_frame, detections)
         return np.eye(2, 3)
@@ -85,8 +89,33 @@ class GMC:
         return H
 
 
+    def applyEcc(self, raw_frame, detections=None):
+        """Reference :78-109.  raw_frame: (H, W, 3) uint8 BGR (ndarray or tensor, host or device); detections are ignored, as in the
+        reference.  Returns a (2, 3) float32 ndarray in down-scaled pixels: the identity on the first frame; after a failed
+        findTransformECC the reference's warning and the map of the last completed iteration."""
+        from b200track.gmc import EccEstimator
+        frame = raw_frame if isinstance(raw_frame, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(raw_frame))
+        h, w = int(frame.shape[0]), int(frame.shape[1])
+        if self._est is None or (self._est.h, self._est.w) != (h, w):
+            if self._est is not None:
+                # the reference keeps its first frame as the template whatever comes later; findTransformECC then refuses frames
+                # of another size.  A new estimator (and template) is the closest this can do.
+                print('Warning: GMC(ecc) frame size changed from %dx%d to %dx%d: new template' % (self._est.w, self._est.h, w, h))
+            self._est = EccEstimator(1, h, w, self.downscale)
+        est = self._est
+        frame = frame.to(est.dev, non_blocking=True).contiguous()[None]
+        warps, stat = est.estimate(frame)
+        self.initializedFirstFrame = True
+        H = warps[0].cpu().numpy().astype(np.float32)
+        self.last_stat = stat.cpu().numpy()[0]
+        if self.last_stat[5] & (L.ECC_FAILED_NAN | L.ECC_FAILED_LAMBDA):
+            print('Warning: find transform failed. Set warp as identity')
+        return H
+
+
 def multi_gmc(stracks, H=np.eye(2, 3)):
-    """Warp the Kalman state of every track in ``stracks`` (reference :250-269) on the GPU."""
+    """Warp the Kalman state of every track in ``stracks`` (reference :250-269) on the GPU.  A float32 H (GMC('ecc')) is promoted as
+    the reference's ``np.kron(np.eye(4, dtype=float), R)`` promotes it: float32 values, float64 arithmetic."""
     if len(stracks) == 0:
         return
     ops = _eng.ops()
