@@ -27,6 +27,32 @@ def _check(lib, rc, what):
 _TUNE_CACHE = {}      # layer signature -> (variant index, tile configuration, record): see DetectorW6._tuned_plan
 
 
+def conv_variants(w, k, s, cin, dtype, stem_row=None):
+    """The addressing variants of one conv launch: [(packed weights, extra ConvPlan arguments)], the default first.  w: the fp32
+    (Cout, Cin, k, k) weight, Cin already padded; stem_row: the row pitch in pixels when the conv reads the padded ReOrg stem buffer."""
+    if stem_row is not None:        # the stem reads the padded ReOrg buffer: row-packed first, generic addressing as the fallback
+        return [(pack_conv_weight_rowpack(w, dtype=dtype), dict(rowpack=True, in_row_pixels=stem_row, x_pixel0=0)),
+                (pack_conv_weight(w, dtype=dtype), dict(in_row_pixels=stem_row, x_pixel0=1)),
+                (pack_conv_weight(w, dtype=dtype), dict(in_row_pixels=stem_row, x_pixel0=1, halo=1))]
+    variants = [(pack_conv_weight(w, dtype=dtype), {})]
+    if k == 3 and s == 1 and cin % 64 == 0:         # halo-tile addressing competes with one-tile-per-tap
+        variants.append((variants[0][0], dict(halo=1)))
+    return variants
+
+
+def conv_candidates(k, s, cin, cout, f32, variants):
+    """Every (variant index, tile configuration) the autotuner times for one conv launch, in timing order: tile width BLOCK_N, one or
+    two 128-pixel sub-tiles per tile (mt), ring depth (0 = as deep as shared memory allows, 2 / 3 = shallow rings) and, for 1x1 layers
+    with whole 128-channel pairs, one or two K chunks per ring stage (kpair), for each addressing variant.  BLOCK_N 32 is offered to
+    layers of at most 32 channels only, where it is the kernel's default tiling.  Some are refused by ``b2t_conv_plan_create`` for a
+    given layer (B2TError); the autotuner skips those."""
+    cout_pad = (cout + 15) // 16 * 16
+    kpairs = (1, 2) if (k == 1 and s == 1 and cin % 128 == 0) else (0,)
+    shapes = [dict(block_n=bn, mt=mt, stages=st, kpair=kp) for bn in (32, 64, 128, 256) for mt in (1, 2) for st in (0, 2, 3) for kp in kpairs
+              if (bn >= 64 or cout_pad <= 32) and bn <= max(64, cout_pad) and 2 * mt * bn <= 512 and not (f32 and mt == 2 and bn > 64)]
+    return [(vi, cfg) for vi in range(len(variants)) for cfg in shapes]
+
+
 class DetectorW6:
     def __init__(self, state_dict, batch=1, img_size=1280, device="cuda:0", conf_thres=0.01, iou_thres=0.45, max_det=300,
                  max_nms=30000, use_graph=True, autotune=True, fuse_pairs=True, act_dtype=torch.float16,
@@ -122,6 +148,10 @@ class DetectorW6:
                 place[i] = (new_buf(hw[i], ch[i]), 0)
         self.place = place
         self.autotune, self.tuned = autotune, {}
+        # one read-only record per conv launch, for per-launch checks: source / destination buffers and channel offsets, every
+        # addressing variant the autotuner offers for it (packed weights, extra ConvPlan arguments), the bias, the geometry, and the
+        # (variant index, tile configuration) this detector runs
+        self.conv_specs = []
         self.ops = []                   # (callable, flops)
         self.keep = []
         sd = state_dict
@@ -140,14 +170,12 @@ class DetectorW6:
             b = torch.cat([sd[nm + ".bias"].to(self.dev, torch.float32) for nm in names], 0).contiguous()
             name = "+".join(names)
             assert w.shape[0] == cout
-            variants = [(pack_conv_weight(w, dtype=act_dtype), {})]
-            if k == 3 and s == 1 and cin % 64 == 0 and self.autotune:      # halo-tile addressing competes with one-tile-per-tap
-                variants.append((variants[0][0], dict(halo=1)))
-            if src[0] is place[0][0] and self.stem_padded:      # the stem reads the padded ReOrg buffer: row-packed first, generic addressing as the fallback
-                variants = [(pack_conv_weight_rowpack(w, dtype=act_dtype), dict(rowpack=True, in_row_pixels=self.stem_row, x_pixel0=0)),
-                            (pack_conv_weight(w, dtype=act_dtype), dict(in_row_pixels=self.stem_row, x_pixel0=1)),
-                            (pack_conv_weight(w, dtype=act_dtype), dict(in_row_pixels=self.stem_row, x_pixel0=1, halo=1))]
-            plan = self._tuned_plan(src, variants, b, dst, hw_in, cin, cout, k, s, act, f32)
+            stem = src[0] is place[0][0] and self.stem_padded
+            variants = conv_variants(w, k, s, cin, act_dtype, self.stem_row if stem else None)
+            # untuned: the first variant the kernel accepts (the stem falls back from row-packed to generic addressing)
+            plan, vi, cfg = self._tuned_plan(src, variants if (self.autotune or stem) else variants[:1], b, dst, hw_in, cin, cout, k, s, act, f32)
+            self.conv_specs.append(dict(name=name, op=len(self.ops), src=src[0], in_coff=src[1], dst=dst[0], out_coff=dst[1], variants=variants, bias=b,
+                                        hw_in=tuple(hw_in), cin=cin, cout=cout, k=k, s=s, act=int(act), f32=bool(f32), chosen=(vi, dict(cfg))))
             self.keep.append(plan)
             flops = 2.0 * self.B * (hw_in[0] // s) * (hw_in[1] // s) * cout * k * k * cin_real
             self.ops.append((plan.run, flops, name))
@@ -255,14 +283,10 @@ class DetectorW6:
     def _tuned_plan(self, src, variants, b, dst, hw_in, cin, cout, k, s, act, f32):
         """Plan-time autotuning: the kernel's best tiling depends on the layer -- tile width BLOCK_N, one or two 128-pixel
         sub-tiles per tile (mt), ring depth (0 = as deep as shared memory allows, 2 / 3 = shallow rings) and the addressing
-        variant -- so each candidate is timed with CUDA events on the real buffers and the fastest kept
-        (tools/conv_layer_bench.py prints the whole table).  ``variants``: [(packed weights, extra ConvPlan arguments)]."""
-        cout_pad = (cout + 15) // 16 * 16
-        shapes = [dict()]
-        if self.autotune:
-            kpairs = (1, 2) if (k == 1 and s == 1 and cin % 128 == 0) else (0,)      # 1x1: one or two K chunks per ring stage
-            shapes = [dict(block_n=bn, mt=mt, stages=st, kpair=kp) for bn in (64, 128, 256) for mt in (1, 2) for st in (0, 2, 3) for kp in kpairs
-                      if bn <= max(64, cout_pad) and 2 * mt * bn <= 512 and not (f32 and mt == 2 and bn > 64)]
+        variant -- so each candidate of ``conv_candidates`` is timed with CUDA events on the real buffers and the fastest kept
+        (tools/conv_layer_bench.py prints the whole table).  ``variants``: [(packed weights, extra ConvPlan arguments)].
+        Returns (plan, variant index, tile configuration); untuned: the first variant accepted with the kernel's default tiling."""
+        cands = conv_candidates(k, s, cin, cout, f32, variants) if self.autotune else [(vi, {}) for vi in range(len(variants))]
         # one tuning per process and layer signature: a second detector of the same shape (tests, the bench's arms) gets the SAME
         # plans without a second tuning pass.  (Every candidate sums each output in the same order -- csrc/b2t_conv.cu -- so the
         # choice changes the time, not the result.)
@@ -271,29 +295,30 @@ class DetectorW6:
         if self.autotune and key in _TUNE_CACHE:
             vi, cfg, rec = _TUNE_CACHE[key]
             self.tuned[len(self.ops)] = dict(rec)
-            return ConvPlan(src[0], variants[vi][0], b, dst[0], self.B, hw_in[0], hw_in[1], cin, src[1], cout, k, s, dst[1], act=act, out_f32=f32, **cfg, **variants[vi][1])
+            return (ConvPlan(src[0], variants[vi][0], b, dst[0], self.B, hw_in[0], hw_in[1], cin, src[1], cout, k, s, dst[1], act=act, out_f32=f32,
+                             **cfg, **variants[vi][1]), vi, cfg)
         best, best_ms = None, None
-        for vi, (wpk, extra) in enumerate(variants):
-            for cfg in shapes:
-                try:
-                    plan = ConvPlan(src[0], wpk, b, dst[0], self.B, hw_in[0], hw_in[1], cin, src[1], cout, k, s, dst[1], act=act, out_f32=f32,
-                                    **cfg, **extra)
-                except L.B2TError:
-                    continue
-                if not self.autotune:
-                    return plan
-                plan.run(); plan.run()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(4):
-                    plan.run()
-                e1.record()
-                torch.cuda.synchronize()
-                ms = e0.elapsed_time(e1)
-                if best_ms is None or ms < best_ms:
-                    best, best_ms = plan, ms
-                    self.tuned[len(self.ops)] = dict(cfg, variant=vi, us=ms * 250.0, **{k_: plan.info[k_] for k_ in ("grid", "stages", "smem")})
-                    _TUNE_CACHE[key] = (vi, dict(cfg), dict(self.tuned[len(self.ops)]))
+        for vi, cfg in cands:
+            wpk, extra = variants[vi]
+            try:
+                plan = ConvPlan(src[0], wpk, b, dst[0], self.B, hw_in[0], hw_in[1], cin, src[1], cout, k, s, dst[1], act=act, out_f32=f32,
+                                **cfg, **extra)
+            except L.B2TError:
+                continue
+            if not self.autotune:
+                return plan, vi, cfg
+            plan.run(); plan.run()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(4):
+                plan.run()
+            e1.record()
+            torch.cuda.synchronize()
+            ms = e0.elapsed_time(e1)
+            if best_ms is None or ms < best_ms:
+                best, best_ms = (plan, vi, dict(cfg)), ms
+                self.tuned[len(self.ops)] = dict(cfg, variant=vi, us=ms * 250.0, **{k_: plan.info[k_] for k_ in ("grid", "stages", "smem")})
+                _TUNE_CACHE[key] = (vi, dict(cfg), dict(self.tuned[len(self.ops)]))
         if best is None:
             raise L.B2TError("no valid conv configuration")
         return best
