@@ -389,6 +389,33 @@ int b2t_batchnorm_batch_stats_segments(const void* x, void* y, const int* offset
 /* b2t_avgpool_l2norm with crop j written to row rowmap[j] of out [rows][512] (:83, :103-104); rowmap[j] < 0: nothing written */
 int b2t_avgpool_l2norm_rows(const void* in, float* out, const int* rowmap, int n, int hw, int c, int act_dtype, void* stream);
 
+/* ---------------------------------------------------------------- StrongSORT's OSNet x0.25 extractor (csrc/b2t_osnet.cu)
+ * tracker/strongsort.py:26-29, :47-89 with tracker/reid_models/OSNet.py in eval mode: BatchNorm folded into the float32 weights the
+ * caller passes (b200track/osnet.py).  Activations NHWC 16-bit (act_dtype), fp32 accumulation in a fixed order, so a crop's result does
+ * not depend on the other crops of the call.  Never allocates, never synchronises; everything is enqueued on `stream`.
+ * b2t_osnet_crops: StrongSORT.reid_preprocess :47-64 for n crops (rows as b2t_reid_crops): float / 255, cv2.resize to out_h rows x
+ *   out_w columns (bilinear), Normalize -> out [n][out_h][out_w][4] (B, G, R, 0). */
+int b2t_osnet_crops(const unsigned char* pixels, const long long* crops, int n, int out_h, int out_w, void* out_nhwc4, int act_dtype, void* stream);
+/* conv 7 x 7 / s2 / p3 (3 -> 16) + bias + ReLU, then max-pool 3 x 3 / s2 / p1: x [n][h][w][pitch] (channels 0..2 read; pitch 4 for
+ * b2t_osnet_crops, 16 for b2t_image_nhwc16), wt [(ky * 7 + kx) * 3 + ci][16], bias [16] -> y [n][h / 4][w / 4][16]; h, w multiples of 4 */
+int b2t_osnet_stem(const void* x, int pitch, const float* wt, const float* bias, int n, int height, int width, void* y, int act_dtype, void* stream);
+/* 1 x 1 conv: y = act(xa . wt[0 : ca] + xb . wt[ca : ca + cb] + bias (+ res)) over the n x height x width pixels; xa [..][ca], xb [..][cb]
+ * (cb = 0 and xb NULL: one input), wt [ca + cb][cout], res NULL or [..][cout]; act = ReLU when relu != 0.  pool != 0: y [n][height / 2]
+ * [width / 2][cout] is the 2 x 2 / s2 average of act(...) (even sides, no res).  Channels multiples of 8, (ca + cb) * cout <= 24576. */
+int b2t_osnet_pointwise(const void* xa, int ca, const void* xb, int cb, const float* wt, const float* bias, const void* res, void* y,
+                        int n, int height, int width, int cout, int relu, int pool, int act_dtype, void* stream);
+/* LightConv3x3: y = ReLU(dwconv3x3_p1(x . w1) + bias); x, y [n][h][w][c] (not in place), w1 [ci][co], dw [dy * 3 + dx][c], bias [c];
+ * 8 <= c <= 64, c % 8 == 0.  The 1 x 1 output is kept in fp32. */
+int b2t_osnet_lightconv(const void* x, const float* w1, const float* dw, const float* bias, void* y, int n, int height, int width, int c,
+                        int act_dtype, void* stream);
+/* OSBlock's x2 = sum_s ChannelGate(s) over the four streams s0..s3 [n][hw][c] with ONE gate: per crop and stream, the channel means ->
+ * fc1 [hidden][c] + b -> ReLU -> fc2 [c][hidden] + b -> sigmoid = g_s; y = g_0 s0 + g_1 s1 + g_2 s2 + g_3 s3.  8 <= c <= 64, c % 8 == 0,
+ * 1 <= hidden <= 16. */
+int b2t_osnet_gate_sum(const void* s0, const void* s1, const void* s2, const void* s3, const float* fc1_w, const float* fc1_b,
+                       const float* fc2_w, const float* fc2_b, void* y, int n, int hw, int c, int hidden, int act_dtype, void* stream);
+/* global average pool of x [n][hw][c] -> Linear + BatchNorm1d (folded: wt [c][m], bias [m]) -> ReLU -> out [n][m] float32; c <= 256 */
+int b2t_osnet_head(const void* x, const float* wt, const float* bias, float* out, int n, int hw, int c, int m, int act_dtype, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

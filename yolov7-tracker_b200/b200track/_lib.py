@@ -117,6 +117,12 @@ SIGNATURES = {
     "b2t_avgpool_l2norm_rows": (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
     "b2t_detect_nms": (_I, [_P, _I, _I, _I, C.c_float, C.c_float, _I, _I, _I, _I, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,
                             _P, _SZ, _P, _P, _P]),
+    "b2t_osnet_crops": (_I, [_P, _P, _I, _I, _I, _P, _I, _P]),
+    "b2t_osnet_stem": (_I, [_P, _I, _P, _P, _I, _I, _I, _P, _I, _P]),
+    "b2t_osnet_pointwise": (_I, [_P, _I, _P, _I, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "b2t_osnet_lightconv": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "b2t_osnet_gate_sum": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "b2t_osnet_head": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
 }
 
 
@@ -135,9 +141,12 @@ REID_SYMBOLS = ["b2t_reid_crops", "b2t_maxpool3x3s2", "b2t_maxpool2x2s2", "b2t_a
                 "b2t_avgpool_l2norm", "b2t_reid_crops_from_dets", "b2t_batchnorm_segments_workspace_bytes", "b2t_batchnorm_batch_stats_segments",
                 "b2t_avgpool_l2norm_rows"]
 
+# StrongSORT's OSNet extractor (csrc/b2t_osnet.cu), also compiled for the host simulator (tests/hostsim/build_sim_osnet.py)
+OSNET_SYMBOLS = [n for n in SIGNATURES if n.startswith("b2t_osnet")]
+
 # the association branch (csrc/b2t_tracker.cu); the rest are the detector's translation units
 TRACKER_SYMBOLS = [n for n in SIGNATURES if not n.startswith(("b2t_conv", "b2t_detect", "b2t_image", "b2t_upsample", "b2t_spp", "b2t_nms", "b2t_letterbox", "b2t_gmc_workspace", "b2t_gmc_reset", "b2t_gmc_estimate", "b2t_gmc_prepare", "b2t_ecc",
-                                                                   "b2t_reid", "b2t_maxpool", "b2t_add_relu", "b2t_avgpool", "b2t_batchnorm"))]
+                                                                   "b2t_reid", "b2t_maxpool", "b2t_add_relu", "b2t_avgpool", "b2t_batchnorm", "b2t_osnet"))]
 
 
 def act_dtype_code(torch_dtype):
