@@ -142,6 +142,8 @@ int b2t_tracker_step_host(b2t_tracker* t, const float* dets_host, const int* det
 /* One sequence's ordered list of tracked (which = 0) or lost (which = 1) tracks -- BaseTracker.tracked_stracks / .lost_stracks,
  * basetrack.py:358-360 -- as rows of b2t_tracker_list_cols() = 13 doubles on the HOST: id, tlwh[4] (STrack.tlwh of the Kalman mean),
  * cls, score, slot, state, is_activated, tracklet_len, start_frame, frame_id.  *n_host = list length (rows beyond max_rows are not copied).
+ * which = 2: every slot of the sequence in slot order (cap rows, free slots included); a slot that left both lists keeps its last
+ * state until a later birth reuses it, so state = 3 (Removed) tells a removal from a duplicate drop.
  * Synchronises the stream. */
 int b2t_tracker_list_cols(void);
 int b2t_tracker_read_list(b2t_tracker* t, int seq, int which, double* rows_host, int max_rows, int* n_host, void* stream);

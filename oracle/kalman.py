@@ -101,7 +101,12 @@ def project(fmt, mean, cov, mean_f32=False, confidence=0.0):
         std = [wp * m[3], wp * m[3], 1e-1, wp * m[3]]
         if fmt == FMT_NSA:
             std = [(1 - confidence) * x for x in std]
-        r = np.square(np.array([float(v) for v in std], dtype=np.float64))
+        if all(isinstance(v, np.float32) for v in std):
+            # NSA, float32 mean, float32 confidence: every term is float32 (1e-1 too, via (1 - conf) * 1e-1), so
+            # np.square runs in float32 (kalman_filter.py:624-626)
+            r = np.square(np.array(std, dtype=np.float32)).astype(np.float64)
+        else:
+            r = np.square(np.array([float(v) for v in std], dtype=np.float64))
     z_hat = np.dot(H, np.asarray(mean, dtype=np.float64))
     s = np.linalg.multi_dot((H, cov, H.T)) + np.diag(r)
     return z_hat, s

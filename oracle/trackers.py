@@ -57,6 +57,7 @@ class TrackerOracle:
         self.tracked = []      # self.tracked_stracks (order matters, q13)
         self.lost = []         # self.lost_stracks
         self.removed_ids = set()   # ids ever appended to self.removed_stracks
+        self.removed_now_ids = []  # ids appended to self.removed_stracks by the last frame, in order (a track can recur)
         self.last_stats = {}
 
     # ------------------------------------------------------------------ helpers
@@ -145,6 +146,7 @@ class TrackerOracle:
     # ------------------------------------------------------------------ list algebra
     def _finish(self, f, lost_now, removed_now, births, refind):
         trk = self.trk
+        self.removed_now_ids = [trk[s].tid for s in removed_now]
         tracked = [s for s in self.tracked if trk[s].state == TRACKED]
         have = {trk[s].tid for s in tracked}
         for s in births + refind:                           # joint_stracks x2 (activated ones already present)
@@ -192,6 +194,15 @@ class TrackerOracle:
             if s not in live:
                 del trk[s]
         return [s for s in tracked if trk[s].activated]
+
+    def list_rows(self, which):
+        """``tracked_stracks`` / ``lost_stracks`` in list order: (int rows id, state, is_activated, start_frame, frame_id,
+        tracklet_len; float64 tlwh)."""
+        slots = self.tracked if which == "tracked" else self.lost
+        rows = np.array([[self.trk[s].tid, self.trk[s].state, int(self.trk[s].activated), self.trk[s].start_frame,
+                          self.trk[s].frame_id, self.trk[s].tracklet_len] for s in slots], np.int64).reshape(-1, 6)
+        tlwh = np.array([np.asarray(self._tlwh(s), np.float64) for s in slots]).reshape(-1, 4)
+        return rows, tlwh
 
     def _emit(self, slots):
         out = []

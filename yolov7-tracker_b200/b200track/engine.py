@@ -218,11 +218,13 @@ class TrackEngine:
 
     def read_list(self, seq, which="tracked"):
         """(n, 13) float64 rows of the sequence's tracked / lost list in the reference's list order: id, tlwh, cls, score, slot,
-        state, is_activated, tracklet_len, start_frame, frame_id (b2t_tracker_read_list)."""
+        state, is_activated, tracklet_len, start_frame, frame_id (b2t_tracker_read_list).  which="slots": every slot in slot
+        order, free ones included (cap rows)."""
         rows = np.zeros((self.cap, 13))
         n = C.c_int(0)
         with torch.cuda.device(self.device):
-            rc = self.lib.b2t_tracker_read_list(self.handle, int(seq), 0 if which == "tracked" else 1, rows.ctypes.data_as(C.c_void_p), self.cap,
+            rc = self.lib.b2t_tracker_read_list(self.handle, int(seq), {"tracked": 0, "lost": 1, "slots": 2}[which],
+                                                rows.ctypes.data_as(C.c_void_p), self.cap,
                                                 C.byref(n), self._stream())
         L.check(self.lib, rc)
         return rows[:n.value].copy()

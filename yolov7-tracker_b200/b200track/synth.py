@@ -113,6 +113,83 @@ def make_reid_stream(seed, n_frames, n_obj=60, feat_dim=64, img=1280, warp_sigma
     return frames, feats, warps
 
 
+def lifecycle_stream(seed, n_frames, n_obj=40, img=1280, conf_thresh=0.2, warp_sigma=0.0):
+    """A stream that walks the tracker through its whole track life cycle: (frames, warps) like ``make_stream``.
+      * a third of the objects are there from frame 1, the others are born at staggered frames; about half leave before the end;
+      * every visible object starts an occlusion with p = 0.03 per frame, 2-45 frames long: the long ones outlive any
+        ``max_time_lost`` up to 30 frames (the track is pruned), the shorter ones are re-found after a gap;
+      * a quarter of the objects are twins of an earlier one (offset by 1-2 px, same size and motion): when one twin is occluded its
+        Lost track sits on top of the other's Tracked one, so ``remove_duplicate_stracks`` drops one of them.  A twin's top-left
+        corner lies a quarter pixel off the integer grid, so its box never has the same area as its sibling's and no track box
+        is exactly as close to both (an exact cost tie would make the assignment solver-dependent);
+      * four frames (never the first) carry no detection at all;
+      * about 5 % of the scores are exactly ``float32(conf)``, ``float32(max(0.15, conf - 0.3))`` or ``float32(conf + 0.1)`` -- the
+        high / low / new-track thresholds the trackers compare against;
+      * warp_sigma > 0: per-frame camera warps with a small rotation and scale and N(0, warp_sigma) translation (boxes move with the
+        translation).
+    Coordinates are integer-rounded (twins' top-left corners: plus a quarter pixel) and clipped, and every frame is sorted by
+    descending score, like ``make_stream``."""
+    rng = np.random.default_rng(seed)
+    n_twin = n_obj // 4
+    n_base = n_obj - n_twin
+    cx = rng.uniform(150, img - 150, n_obj)
+    cy = rng.uniform(150, img - 150, n_obj)
+    w = rng.uniform(24, 80, n_obj)
+    h = rng.uniform(48, 160, n_obj)
+    vx = rng.normal(0, 1, n_obj)
+    vy = rng.normal(0, 1, n_obj)
+    cls = rng.integers(0, 3, n_obj).astype(np.float32)
+    base_score = rng.uniform(0.25, 0.95, n_obj)
+    born = np.where(rng.uniform(0, 1, n_obj) < 1 / 3, 0, rng.integers(1, max(2, int(0.7 * n_frames)), n_obj))
+    life = rng.integers(max(2, n_frames // 4), 2 * n_frames, n_obj)
+    twin_of = rng.choice(n_base, n_twin, replace=False)
+    for k, a in enumerate(twin_of):                            # a twin copies an earlier object's box and motion
+        b = n_base + k
+        cx[b], cy[b] = cx[a] + rng.integers(1, 3), cy[a] + rng.integers(1, 3)
+        w[b], h[b], vx[b], vy[b], cls[b] = w[a], h[a], vx[a], vy[a], cls[a]
+        born[b] = born[a] + rng.integers(0, 8)
+    died = born + life
+    empty = set((1 + rng.choice(n_frames - 1, min(4, n_frames - 1), replace=False)).tolist())
+    ties = np.array([conf_thresh, max(0.15, conf_thresh - 0.3), conf_thresh + 0.1], np.float32)
+    hidden = np.zeros(n_obj, np.int64)
+    frames = []
+    warps = np.zeros((n_frames, 2, 3), dtype=np.float64)
+    warps[:, 0, 0] = warps[:, 1, 1] = 1.0
+    cam = np.zeros(2)
+    for f in range(n_frames):
+        cx += vx
+        cy += vy
+        bx = (cx < 60) | (cx > img - 60)
+        by = (cy < 60) | (cy > img - 60)
+        vx[bx] = -vx[bx]
+        vy[by] = -vy[by]
+        if warp_sigma > 0:
+            t = rng.normal(0, warp_sigma, 2)
+            r, s = rng.normal(0, 5e-4, 2)
+            warps[f] = [[1 + s, -r, t[0]], [r, 1 + s, t[1]]]
+            cam += t
+        alive = (born <= f) & (f < died)
+        start = alive & (hidden == 0) & (rng.uniform(0, 1, n_obj) < 0.03)
+        hidden[start] = rng.integers(2, 46, int(start.sum()))
+        seen = alive & (hidden == 0)
+        hidden[hidden > 0] -= 1
+        jit = rng.normal(0, 1, (n_obj, 4))
+        score = np.clip(base_score + rng.normal(0, 0.1, n_obj), 0.01, 0.99).astype(np.float32)
+        tie = rng.uniform(0, 1, n_obj) < 0.05
+        score[tie] = ties[rng.integers(0, 3, n_obj)[tie]]
+        box = np.stack([cx - w / 2 + jit[:, 0] + cam[0], cy - h / 2 + jit[:, 1] + cam[1],
+                        cx + w / 2 + jit[:, 2] + cam[0], cy + h / 2 + jit[:, 3] + cam[1]], 1)
+        box = np.round(np.clip(box, 0, img))
+        box[n_base:, :2] += 0.25
+        ok = seen & ((box[:, 2] - box[:, 0]) >= 4) & ((box[:, 3] - box[:, 1]) >= 4)
+        if f in empty:
+            ok[:] = False
+        d = np.concatenate([box[ok], score[ok, None], cls[ok, None]], 1).astype(np.float32)
+        order = np.argsort(-d[:, 4], kind="stable")
+        frames.append(np.ascontiguousarray(d[order]))
+    return frames, warps
+
+
 def stream_digest(frames):
     """sha1 of the raw bytes: stored with golden fixtures to detect generator drift."""
     hsh = hashlib.sha1()

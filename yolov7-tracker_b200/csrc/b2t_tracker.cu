@@ -252,14 +252,16 @@ __global__ void read_slot_kernel(TrackState st, int seq, int slot, double* out72
 
 // One of a sequence's ordered slot lists as rows of LIST_COLS doubles: id, tlwh (from the Kalman mean, STrack.tlwh basetrack.py:183-211),
 // cls, score, slot, state, is_activated, tracklet_len, start_frame, frame_id.  out[cap * LIST_COLS] = the list length.
+// which = 2: every slot in slot order (cap rows), free ones included -- a slot that left both lists keeps its last state until a
+// later birth takes it, so the caller can tell a removal (ST_REMOVED) from a duplicate drop.
 constexpr int LIST_COLS = 13;
 template <class T>
 __global__ void read_list_kernel(TrackState st, int fmt, int seq, int which, double* out) {
     SeqView<T> v(st, seq);
-    const int n = which == 0 ? v.ctrl[CTRL_NTRACKED] : v.ctrl[CTRL_NLOST];
+    const int n = which == 0 ? v.ctrl[CTRL_NTRACKED] : which == 1 ? v.ctrl[CTRL_NLOST] : st.cap;
     const int* list = which == 0 ? v.tracked : v.lost;
     for (int k = (int)threadIdx.x; k < n; k += (int)blockDim.x) {
-        const int s = list[k];
+        const int s = which == 2 ? k : list[k];
         T box[4];
         mean_to_tlwh<T>(fmt, v.mean + (size_t)s * 8, (v.flags[s] & 1) != 0, box);
         double* o = out + (size_t)k * LIST_COLS;
@@ -598,7 +600,7 @@ extern "C" int b2t_tracker_step_host(b2t_tracker* t, const float* dets_host, con
 extern "C" int b2t_tracker_list_cols(void) { return LIST_COLS; }
 
 extern "C" int b2t_tracker_read_list(b2t_tracker* t, int seq, int which, double* rows_host, int max_rows, int* n_host, void* stream) {
-    if (!t || seq < 0 || seq >= t->cfg.n_seq || (which != 0 && which != 1) || !rows_host || !n_host || max_rows < 0)
+    if (!t || seq < 0 || seq >= t->cfg.n_seq || which < 0 || which > 2 || !rows_host || !n_host || max_rows < 0)
         return fail(B2T_EINVAL, "b2t_tracker_read_list: bad arguments");
     cudaStream_t s = (cudaStream_t)stream;
     if (t->cfg.dtype == B2T_F64) { auto k = read_list_kernel<double>; B2T_LAUNCH(k, 1, 256, 0, s, t->st, t->cfg.fmt, seq, which, t->d_list); }

@@ -345,7 +345,7 @@ class BaseTracker(object):
         self._last = []
         self._removed = []
         self._watch_removed = False
-        self._alive = {}
+        self._prev_lists = None
 
     # the reference exposes these three lists (basetrack.py:358-360); here they are views of the device-side lists
     @property
@@ -363,14 +363,22 @@ class BaseTracker(object):
 
     @property
     def removed_stracks(self):
-        """Tracks that left both lists.  The reference appends to this list forever; here the bookkeeping (one small device read per
-        frame) starts at the first access, so a caller that wants it from frame 1 reads the property once before tracking."""
-        self._watch_removed = True
+        """The tracks the reference passes to ``mark_removed``, appended in its order (see ``removed_in_step``).  The reference
+        appends to this list forever; here the bookkeeping (three small device reads per frame) starts at the first access, so a
+        caller that wants it from frame 1 reads the property once before tracking."""
+        if not self._watch_removed:
+            self._watch_removed = True
+            self._prev_lists = self._read_lists()
         return list(self._removed)
 
     @removed_stracks.setter
     def removed_stracks(self, v):
         self._removed = list(v)
+
+    def _read_lists(self):
+        if self._engine is None or self.frame_id == 0:
+            return {'tracked': np.zeros((0, 13)), 'lost': np.zeros((0, 13))}
+        return {w: self._engine.read_list(0, w) for w in ('tracked', 'lost')}
 
     def _views(self, which):
         rows = self._engine.read_list(0, which)
@@ -409,7 +417,7 @@ class BaseTracker(object):
                 raise NotImplementedError("use_apperance_model=True is built for BoTSORT only: %s's appearance cost is dense "
                                           "(gamma * IoU + (1 - gamma) * appearance over every pair) and needs another assignment path"
                                           % type(self).__name__)
-            return self._finish_step(self._step_appearance(det_results, ori_img, predict_only))
+            return self._finish_step(self._step_appearance(det_results, ori_img, predict_only), predict_only)
         eng = self._get_engine()
         self.frame_id += 1
         warp = None
@@ -425,9 +433,9 @@ class BaseTracker(object):
                 warp = self._warp(dets, ori_img)
             rows = eng.step_host(warps=None if warp is None else np.asarray(warp, dtype=np.float64).reshape(1, 6),
                                  id_base=[BaseTrack._count], predict_only=predict_only)[0]
-        return self._finish_step(rows)
+        return self._finish_step(rows, predict_only)
 
-    def _finish_step(self, rows):
+    def _finish_step(self, rows, predict_only=False):
         """Track views of the step's output rows; the id counter and the removed-list bookkeeping follow the engine."""
         eng = self._engine
         BaseTrack._count = int(eng.np_stat[0, L.STAT_NEXT_ID])
@@ -435,15 +443,11 @@ class BaseTracker(object):
         fmt = self.opts.kalman_format
         self._last = [_TrackView(eng, 0, rows[i], fmt, self.frame_id) for i in range(rows.shape[0])]
         if self._watch_removed:
-            now = {}
-            for which in ('tracked', 'lost'):
-                for r in eng.read_list(0, which):
-                    now[int(r[0])] = _TrackView(eng, 0, r, fmt, self.frame_id, extra=r[8:13])
-            for tid, view in self._alive.items():
-                if tid not in now:
-                    view.state = TrackState.Removed
-                    self._removed.append(view)
-            self._alive = now
+            if not predict_only:                                   # update_without_detection removes nothing (basetrack.py:489-537)
+                prev = self._prev_lists
+                for r in removed_in_step(prev['tracked'], prev['lost'], eng.read_list(0, 'slots'), self.frame_id, self.max_time_lost):
+                    self._removed.append(_TrackView(eng, 0, r, fmt, self.frame_id, extra=r[8:13]))
+            self._prev_lists = self._read_lists()
         if self.debug_mode:
             print('===========Frame {}=========='.format(self.frame_id))
             print('Tracked: {}'.format([t.track_id for t in self._last]))
@@ -454,6 +458,26 @@ class BaseTracker(object):
 
     def update_without_detection(self, det_results, ori_img):
         return self._step(None, ori_img, predict_only=True)
+
+
+def removed_in_step(prev_tracked, prev_lost, slots, frame_id, max_time_lost):
+    """The rows of the tracks the reference appends to ``removed_stracks`` in one ``update``, in its order (basetrack.py:450-466,
+    bytetrack.py:165-183): first the unconfirmed tracks the last association left unmatched, then every entry of the frame's OLD lost
+    list that has gone more than ``max_time_lost`` frames without an update.  A track pruned in the previous frame is still in that
+    list (the lost list is filtered against the removed list of the frame before), so unless it was re-found it is appended again.
+    A track that ``remove_duplicate_stracks`` drops is not appended.
+    prev_tracked / prev_lost: b2t_tracker_read_list rows at the end of the previous frame; slots: every slot's row after this
+    frame's step (which = 2) -- a slot that left the lists keeps its state until a later frame's birth reuses it."""
+    out = []
+    for r in prev_tracked:
+        s = slots[int(r[7])]
+        if r[9] == 0 and s[8] == TrackState.Removed:
+            out.append(s)
+    for r in prev_lost:
+        s = slots[int(r[7])]
+        if frame_id - s[12] > max_time_lost:
+            out.append(s)
+    return out
 
 
 def joint_stracks(tlista, tlistb):
