@@ -28,7 +28,7 @@ extern "C" {
 
 enum { B2T_F32 = 0, B2T_F64 = 1 };
 enum { B2T_FMT_XYAH = 0, B2T_FMT_XYWH = 1, B2T_FMT_NSA = 2 };
-enum { B2T_SORT = 0, B2T_BYTETRACK = 1, B2T_BOTSORT = 2 };
+enum { B2T_SORT = 0, B2T_BYTETRACK = 1, B2T_BOTSORT = 2, B2T_STRONGSORT = 3 };
 enum { B2T_OK = 0, B2T_EINVAL = -1, B2T_ECUDA = -2, B2T_ECAPACITY = -3, B2T_ENOTBUILT = -4 };
 /* 16-bit activation / weight type of the detector branch.  Both feed wgmma at the same rate with fp32
  * accumulation; fp16 (the reference's own GPU half mode, detect.py:41) carries 3 more mantissa bits than bf16. */
@@ -83,7 +83,7 @@ int b2t_lap_solve(int dtype, const void* cost, int n, int m, int ld, double thre
 typedef struct b2t_tracker b2t_tracker;
 
 typedef struct b2t_tracker_config {
-    int kind;          /* B2T_SORT / B2T_BYTETRACK / B2T_BOTSORT */
+    int kind;          /* B2T_SORT / B2T_BYTETRACK / B2T_BOTSORT / B2T_STRONGSORT */
     int dtype;         /* B2T_F32 / B2T_F64 */
     int fmt;           /* Kalman format */
     int n_seq;         /* sequences per launch */
@@ -101,6 +101,10 @@ typedef struct b2t_tracker_config {
     int feat_dim;
     double theta_iou;   /* associations 1 and 3: the appearance cost counts only where the IoU distance is <= theta_iou (< 1) ... */
     double theta_emb;   /* ... and 0.5 (1 - cos) is <= theta_emb; cost = min(IoU distance, appearance cost).  Defaults 0.5 / 0.25 */
+    /* B2T_STRONGSORT only (StrongSORT.update, strongsort.py:91-250; needs feat_dim > 0, steps through b2t_tracker_step_feat):
+     * associations 1 and 3 cost gamma * IoU distance + (1 - gamma) * Euclidean feature distance, dense (no IoU gate).  In [0, 1],
+     * the reference's default 0.1.  Not read for the other kinds. */
+    double gamma;
 } b2t_tracker_config;
 
 size_t b2t_tracker_state_bytes(const b2t_tracker_config* cfg);
@@ -131,6 +135,10 @@ int b2t_tracker_step(b2t_tracker* t, const float* dets, const int* det_count, co
  * detection's feature; re-activation and low-score updates leave it unchanged. */
 int b2t_tracker_step_feat(b2t_tracker* t, const float* dets, const int* det_count, const float* feats, const double* warps,
                           const int* id_base, double* out, int out_rows, int* stat, int predict_only, void* stream);
+/* Euclidean distances between feature rows, float64: out[b][i][j] = max(0, |a[b][i] - b[b][j]|) for a [batch][n][feat_dim] and
+ * b [batch][m][feat_dim] float32, out [batch][n][m] (matching.embedding_distance(metric='euclidean')).  The kernel B2T_STRONGSORT
+ * runs before each step; |out - exact| <= gamma_{feat_dim+3} * exact with gamma_k = k u / (1 - k u), u = 2^-53. */
+int b2t_feature_distance(const float* a, int n, const float* b, int m, int feat_dim, double* out, int batch, void* stream);
 /* Changes theta_iou / theta_emb for the following steps (the reference reads them as plain attributes every frame). */
 int b2t_tracker_set_thetas(b2t_tracker* t, double theta_iou, double theta_emb);
 /* Copies one slot's smoothed feature (feat_dim floats) to the HOST (lazy STrack.features).  Synchronises the stream. */

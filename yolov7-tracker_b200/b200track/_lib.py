@@ -12,7 +12,7 @@ LIB_PATH = os.path.join(HERE, "libb200track.so")
 
 F32, F64 = 0, 1
 FMT_XYAH, FMT_XYWH, FMT_NSA = 0, 1, 2
-SORT, BYTETRACK, BOTSORT = 0, 1, 2
+SORT, BYTETRACK, BOTSORT, STRONGSORT = 0, 1, 2, 3
 FLAG_MEAN_F32, FLAG_NOT_TRACKED = 1, 2
 ACT_BF16, ACT_F16 = 0, 1
 REID_OVERFLOW, REID_ZERO_SIZE, REID_NEGATIVE = 1, 2, 4       # b2t_reid_crops_from_dets status bits
@@ -23,7 +23,7 @@ ECC_FIRST_FRAME, ECC_CONVERGED, ECC_ITER_CAP, ECC_FAILED_NAN, ECC_FAILED_LAMBDA 
 (STAT_NOUT, STAT_NEXT_ID, STAT_NTRACKED, STAT_NLOST, STAT_ERR, STAT_FRAME, STAT_NPOOL, STAT_NBIRTH,
  STAT_NHI, STAT_NLO, STAT_NEDGE, STAT_NMATCH0) = range(12)
 FMT_BY_NAME = {"default": FMT_XYAH, "botsort": FMT_XYWH, "strongsort": FMT_NSA}
-KIND_BY_NAME = {"sort": SORT, "bytetrack": BYTETRACK, "botsort": BOTSORT}
+KIND_BY_NAME = {"sort": SORT, "bytetrack": BYTETRACK, "botsort": BOTSORT, "strongsort": STRONGSORT}
 
 
 class B2TError(RuntimeError):
@@ -34,7 +34,7 @@ class TrackerConfig(C.Structure):
     _fields_ = [("kind", C.c_int), ("dtype", C.c_int), ("fmt", C.c_int), ("n_seq", C.c_int), ("cap", C.c_int),
                 ("dmax", C.c_int), ("ecap", C.c_int), ("use_gmc", C.c_int), ("track_buffer", C.c_int),
                 ("conf_thresh", C.c_double), ("iou_thresh", C.c_double), ("frame_rate", C.c_double),
-                ("feat_dim", C.c_int), ("theta_iou", C.c_double), ("theta_emb", C.c_double)]
+                ("feat_dim", C.c_int), ("theta_iou", C.c_double), ("theta_emb", C.c_double), ("gamma", C.c_double)]
 
 
 class ConvDesc(C.Structure):
@@ -71,6 +71,7 @@ SIGNATURES = {
     "b2t_tracker_step_host": (_I, [_P, _P, _P, _P, _P, _P, _I, _P, _I, _P]),
     "b2t_tracker_step_feat": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _P, _I, _P]),
     "b2t_tracker_set_thetas": (_I, [_P, _D, _D]),
+    "b2t_feature_distance": (_I, [_P, _I, _P, _I, _I, _P, _I, _P]),
     "b2t_tracker_read_feature": (_I, [_P, _I, _I, _P, _P]),
     "b2t_tracker_read_slot": (_I, [_P, _I, _I, _P, _P, _P]),
     "b2t_tracker_list_cols": (_I, []),

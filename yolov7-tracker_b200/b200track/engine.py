@@ -19,10 +19,12 @@ def _dev_ptr(t):
 class TrackEngine:
     def __init__(self, kind="bytetrack", n_seq=1, dtype="f64", cap=1024, dmax=1024, ecap=None, kalman_format=None,
                  conf_thresh=0.2, iou_thresh=0.5, track_buffer=30, frame_rate=30, use_gmc=True, device="cuda:0",
-                 feat_dim=0, theta_iou=0.5, theta_emb=0.25):
+                 feat_dim=0, theta_iou=0.5, theta_emb=0.25, gamma=0.1):
         """feat_dim > 0 (BoT-SORT only, a multiple of 32 up to 2048): BoT-SORT with appearance features -- every step then takes the
         detections' features (step_device(feats=), step_cuda_dets(feats_list=)) and fuses them into associations 1 and 3 with the
-        gates theta_iou / theta_emb (set_thetas changes them between steps)."""
+        gates theta_iou / theta_emb (set_thetas changes them between steps).
+        kind="strongsort" (StrongSORT.update; feat_dim > 0 required, Kalman format 'strongsort' unless given, as track.py:71 forces):
+        the same feature-carrying steps, with the dense cost gamma * IoU distance + (1 - gamma) * Euclidean feature distance."""
         if not torch.cuda.is_available():
             raise L.B2TError("TrackEngine needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.lib = L.load()
@@ -30,7 +32,7 @@ class TrackEngine:
         if self.device.type == "cuda" and self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())
         if kalman_format is None:
-            kalman_format = "botsort" if kind == "botsort" else "default"      # track.py:68-69
+            kalman_format = {"botsort": "botsort", "strongsort": "strongsort"}.get(kind, "default")      # track.py:68-71
         self.kind, self.kalman_format = kind, kalman_format
         self.dtype = L.F64 if dtype in ("f64", "float64", L.F64) and dtype != L.F32 else L.F32
         if ecap is None:
@@ -41,7 +43,7 @@ class TrackEngine:
                                    n_seq=n_seq, cap=cap, dmax=dmax, ecap=ecap, use_gmc=int(bool(use_gmc)),
                                    track_buffer=int(track_buffer), conf_thresh=float(conf_thresh),
                                    iou_thresh=float(iou_thresh), frame_rate=float(frame_rate), feat_dim=self.feat_dim,
-                                   theta_iou=self.theta_iou, theta_emb=self.theta_emb)
+                                   theta_iou=self.theta_iou, theta_emb=self.theta_emb, gamma=float(gamma))
         nbytes = self.lib.b2t_tracker_state_bytes(C.byref(self.cfg))
         if nbytes == 0:
             raise L.B2TError((self.lib.b2t_last_error() or b"").decode())

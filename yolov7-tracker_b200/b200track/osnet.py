@@ -286,3 +286,63 @@ class OsnetExtractor:
             self._run(net, "x16")
         self.last_net = net
         return net["feat"][:n]
+
+
+class OsnetSegments:
+    """StrongSORT's crops of S sequences in ONE OSNet pass at a fixed capacity of `cap` crops, with nothing in a step that depends on a
+    host-side count (TrackingPipeline with a StrongSORT engine).  ``cut`` builds the crop list on the device from the NMS output with
+    b2t_reid_crops_from_dets -- the rows with score > det_thresh, StrongSORT's strict test (strongsort.py:118), by passing the next
+    float32 above it to that kernel's >= test; ``run`` cuts and runs the network over all `cap` rows (padding rows repeat a valid crop)
+    and scatters the feature of crop j to row rowmap[j] of ``feats`` (S, dmax, 512), the tensor TrackEngine.step_device(feats=) takes.
+    An OSNet feature does not depend on the other crops of the pass (eval-mode BatchNorm), so one pass serves every sequence."""
+
+    def __init__(self, ext, n_seq, dmax, cap):
+        if n_seq < 1 or dmax < 1 or cap < 1:
+            raise L.B2TError("OsnetSegments: n_seq, dmax and cap must be >= 1 (got %d, %d, %d)" % (n_seq, dmax, cap))
+        self.ext, self.S, self.dmax, self.cap = ext, int(n_seq), int(dmax), int(cap)
+        dev = ext.dev
+        with torch.cuda.device(dev):
+            self.crops = torch.zeros((self.cap, 4), dtype=torch.int64, device=dev)
+            self.offsets = torch.zeros(self.S + 1, dtype=torch.int32, device=dev)
+            self.rowmap = torch.full((self.cap,), -1, dtype=torch.int32, device=dev)
+            self.status = torch.zeros(self.S + 1, dtype=torch.int32, device=dev)
+            self._rows = torch.zeros((self.S * self.dmax + 1, FEATURE_DIM), dtype=torch.float32, device=dev)   # last row: padding sink
+            self.feats = self._rows[: self.S * self.dmax].view(self.S, self.dmax, FEATURE_DIM)
+
+    def capture(self):
+        """Builds the network at this capacity and captures its graph (synchronises the device): a pass over 1 x 1 crops."""
+        crops = torch.tensor([[0, 3, 1, 1]], dtype=torch.int64, device=self.ext.dev).repeat(self.cap, 1)
+        self.ext.features(torch.zeros(3, dtype=torch.uint8, device=self.ext.dev), crops)
+        torch.cuda.synchronize(self.ext.dev)
+
+    def cut(self, frames, dets, det_count, det_thresh):
+        """On the current stream: frames (S, H, W, 3) uint8 device tensor, dets (S, dmax, 6) float32, det_count (S,) int32 (the
+        detector's out / out_count); det_thresh: the tracker's conf_thresh."""
+        if tuple(dets.shape) != (self.S, self.dmax, 6) or dets.dtype != torch.float32 or det_count.dtype != torch.int32 or tuple(det_count.shape) != (self.S,):
+            raise L.B2TError("OsnetSegments.cut: dets must be float32 (%d, %d, 6) and det_count int32 (%d,)" % (self.S, self.dmax, self.S))
+        if frames.dtype != torch.uint8 or frames.dim() != 4 or int(frames.shape[0]) != self.S or int(frames.shape[3]) != 3 or not frames.is_contiguous():
+            raise L.B2TError("OsnetSegments.cut: frames must be a contiguous uint8 (%d, H, W, 3) tensor" % self.S)
+        H, W = int(frames.shape[1]), int(frames.shape[2])
+        strict = float(np.nextafter(np.float32(det_thresh), np.float32(np.inf)))
+        rc = self.ext.lib.b2t_reid_crops_from_dets(dets.data_ptr(), det_count.data_ptr(), self.S, self.dmax, strict, H, W, self.cap,
+                                                   self.crops.data_ptr(), self.offsets.data_ptr(), self.rowmap.data_ptr(),
+                                                   self.status.data_ptr(), self.ext._stream())
+        self.ext._check(rc, "b2t_reid_crops_from_dets")
+
+    def run(self, frames):
+        """On the current stream, while `frames` (the buffer ``cut`` saw) is still valid: crops + network + scatter to ``feats``."""
+        f = self.ext.features(frames, self.crops)
+        sink = self.S * self.dmax
+        idx = torch.where(self.rowmap >= 0, self.rowmap, torch.full_like(self.rowmap, sink)).long()
+        self._rows.index_copy_(0, idx, f)
+
+    def raise_for_status(self, status):
+        """status: the (S + 1,) status words read back -> B2TError naming the first refused condition and sequence."""
+        for s in range(self.S):
+            bits = int(status[s])
+            if bits & L.REID_OVERFLOW:
+                raise L.B2TError("OSNet: sequence %d: the crops of this step (%d in all sequences) exceed reid_cap = %d" % (s, int(status[self.S]), self.cap))
+            if bits & L.REID_ZERO_SIZE:
+                raise L.B2TError("OSNet: sequence %d: a detection with score > det_thresh gives an empty crop (cv2.resize raises on it in the reference)" % s)
+            if bits & L.REID_NEGATIVE:
+                raise L.B2TError("OSNet: sequence %d: a detection with score > det_thresh has a negative coordinate after int() (the reference's slice would wrap)" % s)

@@ -14,6 +14,9 @@ the PREVIOUS call (one frame of latency, same results); ``flush()`` returns the 
 With ``reid=`` (BoT-SORT with appearance) the tracker stream also builds the crop list of every sequence's det_high rows from the NMS
 output, cuts the crops out of the detector's uint8 frame buffer (after which the next copy may overwrite it), runs the extractor's graph
 with BatchNorm statistics per sequence, and hands the features to the tracker step -- no host round trip.
+With a StrongSORT engine (``reid=`` an ``OsnetExtractor``, ``gmc=`` an ``EccEstimator`` or None) the tracker stream estimates the
+ECC warps from the uint8 frames, builds the crop list of the rows with score > conf_thresh from the NMS output, runs one OSNet pass
+over all sequences' crops and hands the rows to the StrongSORT step.
 """
 import torch
 
@@ -30,7 +33,10 @@ class TrackingPipeline:
         with feat_dim = 512): one extractor pass per step over the det_high crops of all sequences, each sequence's crops normalised
         with its own batch statistics as the reference's one-tracker-per-sequence calls do.  reid_cap: crops per pass (default
         n_seq * dmax, which cannot overflow); a step with more det_high rows raises B2TError when its tracks are collected.
-        Frames must then be uint8 (the crops come from det.src_u8)."""
+        Frames must then be uint8 (the crops come from det.src_u8).
+        StrongSORT (engine kind "strongsort", feat_dim 512): reid must be a ``b200track.osnet.OsnetExtractor`` and gmc an
+        ``EccEstimator`` for the source-frame size, or None for use_ECC=False; reid_cap defaults to min(n_seq * dmax, 1024).  A
+        StrongSORT engine with a ReidExtractor or a GmcEstimator, and an OsnetExtractor or EccEstimator with another engine, raise."""
         self.dets = list(detector) if isinstance(detector, (list, tuple)) else [detector]
         if len(self.dets) not in (1, 2):
             raise L.B2TError("TrackingPipeline takes one detector or two twins")
@@ -42,10 +48,35 @@ class TrackingPipeline:
                 raise L.B2TError("TrackEngine(n_seq=%d, dmax=%d) does not match DetectorW6(batch=%d, max_det=%d)" % (engine.S, engine.dmax, d.B, d.max_det))
         if gmc is not None and gmc.S != det.B:
             raise L.B2TError("GmcEstimator(n_seq=%d) does not match DetectorW6(batch=%d)" % (gmc.S, det.B))
+        from .gmc import EccEstimator
+        from .osnet import OsnetExtractor, OsnetSegments
+        ss = engine.kind == "strongsort"
+        # StrongSORT pairs with GMC('ecc') and OSNet (strongsort.py:26-33), BoT-SORT with GMC('orb') and the DeepSORT extractor
+        if ss and (reid is None or not isinstance(reid, OsnetExtractor)):
+            raise L.B2TError("TrackingPipeline: a StrongSORT engine needs reid=OsnetExtractor (got %s)" % type(reid).__name__)
+        if isinstance(reid, OsnetExtractor) and not ss:
+            raise L.B2TError("TrackingPipeline(reid=OsnetExtractor): StrongSORT's extractor needs a StrongSORT engine (got %s)" % engine.kind)
+        if gmc is not None and ss != isinstance(gmc, EccEstimator):
+            raise L.B2TError("TrackingPipeline: %s takes %s for gmc= (got %s)" % ("StrongSORT" if ss else engine.kind,
+                             "an EccEstimator" if ss else "a GmcEstimator", type(gmc).__name__))
+        self.ecc, self.ss = (gmc if ss else None), ss
         dev = det.dev
         self.dev = dev
         self.reid, self.reid_net = reid, None
-        if reid is not None:
+        if ss:
+            if engine.feat_dim != 512:
+                raise L.B2TError("TrackingPipeline(reid=OsnetExtractor): the engine must have feat_dim=512 (got %d)" % engine.feat_dim)
+            idx = lambda d: torch.device(d).index if torch.device(d).index is not None else torch.cuda.current_device()      # noqa: E731
+            if not (idx(reid.dev) == idx(dev) == idx(engine.device)):
+                raise L.B2TError("TrackingPipeline(reid=): extractor on %s, detector on %s, engine on %s" % (reid.dev, dev, engine.device))
+            # every crop of the pass costs full compute: the default stays at 1024 crops per step, not n_seq * dmax
+            cap = min(engine.S * engine.dmax, 1024) if reid_cap is None else int(reid_cap)
+            if cap < 1:
+                raise L.B2TError("TrackingPipeline: reid_cap must be >= 1, got %d" % cap)
+            self.reid_net = OsnetSegments(reid, engine.S, engine.dmax, cap)
+            self.reid_net.capture()
+            self.h_rstat = [torch.zeros(engine.S + 1, dtype=torch.int32).pin_memory() for _ in range(2)]
+        elif reid is not None:
             if engine.kind != "botsort" or engine.feat_dim != 512:
                 raise L.B2TError("TrackingPipeline(reid=): the engine must be BoT-SORT with feat_dim=512 (got %s, feat_dim=%d)" % (engine.kind, engine.feat_dim))
             idx = lambda d: torch.device(d).index if torch.device(d).index is not None else torch.cuda.current_device()      # noqa: E731
@@ -129,13 +160,13 @@ class TrackingPipeline:
         with torch.cuda.stream(s_in):
             if self.twin:
                 s_in.wait_event(self.ev_fwd_done[i])
-                if self.gmc is not None:
+                if self.gmc is not None and self.ecc is None:
                     s_in.wait_event(self.ev_out_free[i])                       # the estimate of two frames ago has read this slot's planes
             else:
                 s_in.wait_event(self.ev_in_ready[i])
             if u8:
                 det.ingest_u8_launch()                                         # letterbox + RGB + /255 + ReOrg + 16-bit NHWC
-                if self.gmc is not None:
+                if self.gmc is not None and self.ecc is None:
                     self.gmc.prepare(det.src_u8, k)                            # gray / FAST scores / smoothed image while the frame buffer is valid
             else:
                 det.ops[0][0]()                                                # ReOrg + 16-bit NHWC of the float tensor
@@ -160,16 +191,24 @@ class TrackingPipeline:
         with torch.cuda.stream(self.s_trk):
             self.s_trk.wait_event(self.ev_nms_done[i])
             rn = self.reid_net
-            if rn is not None:
+            if self.ss:
+                # StrongSORT: ECC warps of the pool, the crops of the rows with score > conf_thresh, one OSNet pass; det.src_u8 is free after
+                if self.ecc is not None:
+                    warps = self.ecc.estimate(det.src_u8)[0].view(eng.S, 6)
+                rn.cut(det.src_u8, det.out, det.out_count, float(eng.cfg.conf_thresh))
+                rn.run(det.src_u8)
+                self.ev_src_free[i].record(self.s_trk)
+            elif rn is not None:
                 # crop list of every sequence's det_high rows + the crops cut out of the frames: det.src_u8 is free after this
                 rn.cut(det.src_u8, det.out, det.out_count, float(eng.cfg.conf_thresh))
                 self.ev_src_free[i].record(self.s_trk)
-            if self.gmc is not None and u8:
+            if self.gmc is not None and self.ecc is None and u8:
                 # key points outside the boxes of the high-score detections (botsort.py:380), matching, RANSAC -> warps on the device
                 w23, _ = self.gmc.estimate_prepared(k, det.out, det.out_count, det_thresh=float(eng.cfg.conf_thresh))
                 warps = w23.view(eng.S, 6)
             if rn is not None:
-                rn.run()                                                       # extractor graph -> rn.feats rows s * dmax + i
+                if not self.ss:
+                    rn.run()                                                   # extractor graph -> rn.feats rows s * dmax + i
                 eng.step_device(det.out, det.out_count, self.t_out, self.t_stat, warps=warps, feats=rn.feats)
             else:
                 eng.step_device(det.out, det.out_count, self.t_out, self.t_stat, warps=warps)

@@ -113,6 +113,68 @@ def make_reid_stream(seed, n_frames, n_obj=60, feat_dim=64, img=1280, warp_sigma
     return frames, feats, warps
 
 
+def make_strongsort_stream(seed, n_frames, n_obj=40, feat_dim=64, img=1280, warp_sigma=1.0, occl=0.04, jump=0.03):
+    """A stream for StrongSORT: (frames, feats, warps), feats[f] row-aligned with frames[f].
+      * every object has a seeded unit identity vector; a detection's feature is that vector plus noise, times a scale in [0.85, 1.15],
+        so the raw features have norms around 1 and the Euclidean appearance term decides matches (StrongSORT compares raw detection
+        rows with unit track rows, q19);
+      * an object jumps by 1.5-3 box widths with probability `jump` per frame (0.4 on the frame after it enters), so that only
+        appearance can match it (zero IoU), and
+        goes unseen for 2-8 frames with probability `occl` (Lost tracks, re-activated wherever they reappear);
+      * objects enter at staggered frames, so that unconfirmed tracks meet association 3 throughout the stream;
+      * scores lie in [0.05, 0.95]: some rows fall below det_thresh (StrongSORT drops them) and some between det_thresh and
+        det_thresh + 0.1 (no birth).
+    Coordinates are not rounded, so no two costs tie exactly."""
+    rng = np.random.default_rng(seed)
+    cx = rng.uniform(150, img - 150, n_obj)
+    cy = rng.uniform(150, img - 150, n_obj)
+    w = rng.uniform(30, 70, n_obj)
+    h = rng.uniform(60, 140, n_obj)
+    vx = rng.normal(0, 2.0, n_obj)
+    vy = rng.normal(0, 2.0, n_obj)
+    ident = rng.normal(0, 1, (n_obj, feat_dim))
+    ident /= np.linalg.norm(ident, axis=1, keepdims=True)
+    enter = rng.integers(0, max(1, n_frames // 2), n_obj)
+    enter[: n_obj // 3] = 0
+    base_score = rng.uniform(0.3, 0.95, n_obj)
+    hidden = np.zeros(n_obj, np.int64)
+    frames, feats = [], []
+    warps = np.zeros((n_frames, 2, 3), dtype=np.float64)
+    warps[:, 0, 0] = warps[:, 1, 1] = 1.0
+    cam = np.zeros(2)
+    for f in range(n_frames):
+        jmp = rng.uniform(0, 1, n_obj) < np.where(f == enter + 1, 0.4, jump)     # often right after a birth (association 3)
+        ang = rng.uniform(0, 2 * np.pi, n_obj)
+        dist = rng.uniform(1.5, 3.0, n_obj) * w
+        cx += vx + jmp * dist * np.cos(ang)
+        cy += vy + jmp * dist * np.sin(ang)
+        cx = np.clip(cx, 80, img - 80)
+        cy = np.clip(cy, 80, img - 80)
+        t = rng.normal(0, warp_sigma, 2)
+        warps[f, :, 2] = t
+        cam += t
+        start = (hidden == 0) & (rng.uniform(0, 1, n_obj) < occl)
+        hidden[start] = rng.integers(2, 9, int(start.sum()))
+        seen = (hidden == 0) & (enter <= f)
+        hidden[hidden > 0] -= 1
+        jit = rng.normal(0, 1.0, (n_obj, 4))
+        score = np.clip(base_score + rng.normal(0, 0.05, n_obj), 0.05, 0.95)
+        score = np.where(rng.uniform(0, 1, n_obj) < 0.1, rng.uniform(0.05, 0.2, n_obj), score)
+        x1 = cx - w / 2 + jit[:, 0] + cam[0]
+        y1 = cy - h / 2 + jit[:, 1] + cam[1]
+        x2 = cx + w / 2 + jit[:, 2] + cam[0]
+        y2 = cy + h / 2 + jit[:, 3] + cam[1]
+        box = np.clip(np.stack([x1, y1, x2, y2], 1), 0, img)
+        ok = seen & ((box[:, 2] - box[:, 0]) >= 4) & ((box[:, 3] - box[:, 1]) >= 4)
+        d = np.concatenate([box[ok], score[ok, None], (np.arange(n_obj) % 3)[ok, None]], 1).astype(np.float32)
+        k = int(ok.sum())
+        fe = (ident[ok] + rng.normal(0, 0.25 / np.sqrt(feat_dim), (k, feat_dim))) * rng.uniform(0.85, 1.15, (k, 1))
+        order = rng.permutation(k)
+        frames.append(np.ascontiguousarray(d[order]))
+        feats.append(np.ascontiguousarray(fe.astype(np.float32)[order]))
+    return frames, feats, warps
+
+
 def lifecycle_stream(seed, n_frames, n_obj=40, img=1280, conf_thresh=0.2, warp_sigma=0.0):
     """A stream that walks the tracker through its whole track life cycle: (frames, warps) like ``make_stream``.
       * a third of the objects are there from frame 1, the others are born at staggered frames; about half leave before the end;

@@ -364,6 +364,65 @@ B2T_DEVNI bool build_csr(SeqView<T>& v, StepSmem<T>& sm, int n, int m, T thresh,
     return fits;
 }
 
+// StrongSORT's fused cost (strongsort.py:150-157, :206-208): gamma * IoU distance + (1 - gamma) * App, with App the Euclidean distance
+// between the track's feature row and the detection's (dist, written by feat_dist_kernel before the step).  The cost is dense and not
+// gated: a pair that does not overlap (IoU distance 1) still qualifies when App < (thresh - gamma) / (1 - gamma), so the overlap
+// traversal of build_csr cannot find the candidates.  Every (row, column) pair is evaluated instead -- one warp per row, once to count
+// and once to list, O(rows x cols) IoUs and distance loads, no feature work -- and exactly the pairs with cost < thresh are listed, in
+// the same row-contiguous CSR layout (shared-memory mirror first, then the global edge workspace).
+struct DenseCtx {
+    const int* row_slot;    // [n] track slot of each row
+    const int* col_det;     // [m] detection row of each column
+    const double* dist;     // this sequence's [cap][ld] distances: row = slot, column = detection row
+    int ld;
+    double gamma;
+};
+
+template <class T>
+B2T_DEVNI bool build_csr_dense(SeqView<T>& v, StepSmem<T>& sm, int n, int m, T thresh, const DenseCtx& dc) {
+    const int tid = (int)threadIdx.x, nthr = (int)blockDim.x, lane = lane_id();
+    const T g = (T)dc.gamma, g1 = (T)(1.0 - dc.gamma);     // (1. - self.gamma) is a Python float
+    auto cost_of = [&](int i, int j) {
+        const T iou_d = (T)1 - iou_plus1<T>(sm.rowbox + 4 * i, sm.colbox + 4 * j);
+        const T app = (T)dc.dist[(size_t)dc.row_slot[i] * dc.ld + dc.col_det[j]];
+        return g * iou_d + g1 * app;
+    };
+    for (int i = warp_id(); i < n; i += num_warps()) {
+        int cnt = 0;
+        for (int j0 = 0; j0 < m; j0 += 32) {
+            const int j = j0 + lane;
+            cnt += __popc(__ballot_sync(B2T_FULL, j < m && cost_of(i, j) < thresh));
+        }
+        if (lane == 0) { sm.rcnt[i] = cnt; sm.rstart[i] = cnt; }
+    }
+    if (tid == 0) sm.rstart[n] = 0;
+    __syncthreads();
+    const int total = block_exscan(sm.rstart, n + 1, sm.lap.scratch);
+    const bool fits = total <= v.ecap;
+    if (tid == 0) { sm.misc[50] = total; sm.misc[51] = fits ? 0 : 1; }
+    if (fits) {
+        for (int i = warp_id(); i < n; i += num_warps()) {
+            int pos = sm.rstart[i];
+            const bool to_smem = pos + sm.rcnt[i] <= sm.esm;
+            int* ocol = to_smem ? sm.se_col : v.e_col;
+            int* orow = to_smem ? sm.se_row : v.e_row;
+            T* ocost = to_smem ? sm.se_cost : v.e_cost;
+            for (int j0 = 0; j0 < m; j0 += 32) {
+                const int j = j0 + lane;
+                const T cst = j < m ? cost_of(i, j) : (T)1;
+                const bool f = j < m && cst < thresh;
+                const unsigned bal = __ballot_sync(B2T_FULL, f);
+                if (f) { const int q = pos + __popc(bal & lanemask_lt()); ocol[q] = j; orow[q] = i; ocost[q] = cst; }
+                pos += __popc(bal);
+            }
+        }
+    } else {
+        for (int i = tid; i < n; i += nthr) sm.rcnt[i] = 0;
+    }
+    __syncthreads();
+    return fits;
+}
+
 template <class T> struct StepCtx {
     SeqView<T> v;
     StepSmem<T> sm;
@@ -388,11 +447,15 @@ template <class T> B2T_DEV LapCsr<T> step_csr(StepCtx<T>& c, int w2_base = 0, in
     return g;
 }
 
-template <class T> B2T_DEVNI void associate(StepCtx<T>& c, int n, int m, T thresh, int* err, long long* tsplit, int* dbg = nullptr,
-                                             const AppCtx* app = nullptr) {
+// DENSE: the candidates are every pair whose StrongSORT cost is below thresh (build_csr_dense, *dense), not the overlapping ones.
+template <class T, bool DENSE = false> B2T_DEVNI void associate(StepCtx<T>& c, int n, int m, T thresh, int* err, long long* tsplit,
+                                                                int* dbg = nullptr, const AppCtx* app = nullptr,
+                                                                const DenseCtx* dense = nullptr) {
     StepSmem<T>& sm = c.sm;
     long long dt = phase_clock();
-    const bool ok = build_csr<T>(c.v, sm, n, m, thresh, dbg, &dt, app);
+    bool ok;
+    if constexpr (DENSE) ok = build_csr_dense<T>(c.v, sm, n, m, thresh, *dense);
+    else ok = build_csr<T>(c.v, sm, n, m, thresh, dbg, &dt, app);
     if (!ok && threadIdx.x == 0) *err |= ERR_EDGES;
     // The rows that did not fit the shared-memory edge mirror live in the global edge workspace.  rowbox / colbox are dead from
     // here to the next association (each one refills them): the first spilled rows are copied into that memory, so that the
@@ -521,10 +584,13 @@ B2T_DEVNI void copy_features(float* tfeat, int D, const int* slots, const int* d
 
 // APP: the BoT-SORT-with-ReID instantiation (feat_dim > 0).  The IoU-only trackers run the APP = false one, which compiles to the
 // same code as without appearance support.
-template <class T, bool APP>
+// SS (with APP): StrongSORT.update (strongsort.py:91-250).  dist_all [S][cap][dmax] holds the Euclidean distances feat_dist_kernel
+// computed for this frame (tracked and lost lists at frame start x detection rows); gamma weighs the IoU distance in the fused cost.
+template <class T, bool APP, bool SS = false>
 B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq, const float* dets_all,
                             const int* det_count, const float* feats_all, const double* warps, const int* id_base, double* out_all,
-                            int out_rows, int* stat_all, unsigned char* smem_raw) {
+                            int out_rows, int* stat_all, unsigned char* smem_raw, const double* dist_all = nullptr,
+                            double gamma = 0.0) {
     StepCtx<T> c(st, seq, prm);
     Arena arena(smem_raw);
     c.sm.carve(arena, st.cap, st.dmax, st.esm);
@@ -574,7 +640,7 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         return d[3] - d[1] != 0.f && (p.fmt != FMT_XYWH || d[2] - d[0] != 0.f);
     };
     int nhi, nlo;
-    if (p.kind == KIND_SORT) {
+    if (SS || p.kind == KIND_SORT) {      // StrongSORT: score > det_thresh, no low-score set (strongsort.py:118)
         nhi = block_compact(nd, [&](int i) { return dets[6 * i + 4] > p.det_thresh && has_area(i); }, sm.hi, sm.misc);
         nlo = 0;
     } else {
@@ -604,7 +670,9 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
     B2T_PHASE(1);
     // ---- P2: Kalman predict (+ camera-motion warp) for the pool, warp for the unconfirmed
     T warp6[6];
-    const bool gmc = p.use_gmc && p.kind == KIND_BOTSORT && warps != nullptr && !p.predict_only;
+    // StrongSORT warps the pool only, BEFORE the prediction (strongsort.py:140-147); multi_gmc leaves float64 means, so the process
+    // noise is then evaluated in float64
+    const bool gmc = p.use_gmc && (SS || p.kind == KIND_BOTSORT) && warps != nullptr && !p.predict_only;
     if (gmc) for (int q = 0; q < 6; ++q) warp6[q] = (T)warps[(size_t)seq * 6 + q];
     {
         const int r = lane_id() & 7, grp = lane_id() >> 3;
@@ -615,14 +683,15 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
             KRow<T> kr;
             if (on) kf_load<T>(kr, v.mean + (size_t)slot * 8, v.cov + (size_t)slot * 64, r);
             else { kr.m = (T)0; for (int j = 0; j < 8; ++j) kr.p[j] = (T)0; }
-            kf_predict<T>(kr, r, p.fmt, on && sm.pstate[k] != ST_TRACKED, q_f32);
-            if (gmc) kf_gmc<T>(kr, r, warp6);
+            if constexpr (SS) { if (gmc) kf_gmc<T>(kr, r, warp6); }
+            kf_predict<T>(kr, r, p.fmt, on && sm.pstate[k] != ST_TRACKED, (SS && gmc) ? false : q_f32);
+            if (!SS && gmc) kf_gmc<T>(kr, r, warp6);
             if (on) {
                 kf_store<T>(kr, v.mean + (size_t)slot * 8, v.cov + (size_t)slot * 64, r);
                 if (r == 0) v.flags[slot] &= ~1;
             }
         }
-        if (gmc) {
+        if (!SS && gmc) {
             for (int base = warp_id() * 4; base < nunc; base += num_warps() * 4) {
                 const int k = base + grp;
                 const bool on = k < nunc;
@@ -651,7 +720,16 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         B2T_PHASE(3);
         long long tsplit = tprev;
         const AppCtx app1 = {sm.pool, sm.hi, feats, p.theta_iou, p.theta_emb};
-        associate<T>(c, npool, nhi, (T)p.t1, err, &tsplit, stat + STAT_SUB0, feats ? &app1 : nullptr);
+        // StrongSORT: per pool row, what this frame did to it (read by the list algebra, P9): 1 updated in association 1,
+        // 2 re-activated in association 1, 4 updated in association 2, 8 marked lost by q18
+        const double* dist = SS ? dist_all + (size_t)seq * cap * st.dmax : nullptr;
+        if constexpr (SS) {
+            for (int k = tid; k < npool; k += nthr) sm.dupa[k] = 0;
+            const DenseCtx d1 = {sm.pool, sm.hi, dist, st.dmax, gamma};
+            associate<T, true>(c, npool, nhi, (T)p.t1, err, &tsplit, stat + STAT_SUB0, nullptr, &d1);
+        } else {
+            associate<T>(c, npool, nhi, (T)p.t1, err, &tsplit, stat + STAT_SUB0, feats ? &app1 : nullptr);
+        }
         if (tid == 0) { stat[STAT_PHASE0 + 4] = (int)(tsplit - tprev); tprev = tsplit;
                         stat[12] = sm.lap.scratch[45]; stat[13] = sm.lap.scratch[41]; stat[14] = sm.lap.scratch[43]; stat[15] = sm.misc[50]; }
         B2T_PHASE(5);
@@ -667,7 +745,7 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         int nut;
         if (sort)
             nut = block_compact(npool, [&](int i) { return x[i] < 0 && sm.pstate[i] == ST_TRACKED; }, sm.ut, sm.misc);
-        else if (p.kind == KIND_BYTETRACK)
+        else if (SS || p.kind == KIND_BYTETRACK)     // strongsort.py:183: only the Tracked leftovers go on
             nut = block_compact(npool, [&](int i) { return x[i] < 0 && sm.pstate[i] == ST_TRACKED; }, sm.ut, sm.misc);
         else
             nut = block_compact(npool, [&](int i) { return x[i] < 0; }, sm.ut, sm.misc);
@@ -681,7 +759,44 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         apply_matches<T>(c, sm.pool, npool, dets, sm.ntr, sm.used);
         if (feats) ema_features(v.feat, v.feat_dim, sm.pool, npool, feats, sm.ntr, sm.used);
         B2T_PHASE(6);
-        if (sort) {
+        if constexpr (SS) {
+            for (int k = tid; k < npool; k += nthr)
+                if (x[k] >= 0) sm.dupa[k] = sm.pstate[k] == ST_TRACKED ? 1 : 2;
+            // ---- association 2 (strongsort.py:180-198): u_tracks0 (Tracked leftovers) x the leftover detections, IoU only, 0.5
+            for (int k = tid; k < nut; k += nthr) sm.nlo[k] = sm.pool[sm.ut[k]];
+            __syncthreads();
+            fill_track_boxes<T>(v, p.fmt, sm.nlo, nut, sm.rowbox);
+            for (int k = tid; k < nud0; k += nthr)
+                for (int q = 0; q < 4; ++q) sm.colbox[4 * k + q] = sm.detbox[4 * sm.udets0[k] + q];
+            __syncthreads();
+            associate<T>(c, nut, nud0, (T)p.t2, err, nullptr);
+            for (int k = tid; k < nut; k += nthr) {
+                const int xx = x[k];
+                sm.ntr[k] = xx >= 0 ? sm.udets0[xx] : -1;
+                sm.used[k] = 0;
+                if (xx >= 0) sm.dupa[sm.ut[k]] |= 4;
+            }
+            __syncthreads();
+            apply_matches<T>(c, sm.nlo, nut, dets, sm.ntr, sm.used);
+            ema_features(v.feat, v.feat_dim, sm.nlo, nut, feats, sm.ntr, sm.used);    // every StrongSORT detection has a feature
+            // q18 (strongsort.py:195-198): u_tracks1_idx indexes u_tracks0, but the track marked lost is strack_pool[idx] -- possibly
+            // one updated or re-activated this frame.  The track that really went unmatched stays Tracked.
+            for (int k = tid; k < nut; k += nthr)
+                if (x[k] < 0) { v.state[sm.pool[k]] = ST_LOST; sm.dupa[k] |= 8; }
+            __syncthreads();
+            // lost_stracks: the marked rows, except a Lost track that was not re-found -- it is still on the lost list, where
+            // sub_stracks' id dict keeps its old position
+            nlostnow = block_compact(nut, [&](int k) { return x[k] < 0 && !(sm.pstate[k] == ST_LOST && sm.dupa[k] == 8); },
+                                     sm.ut, sm.misc);
+            for (int k = tid; k < nlostnow; k += nthr) sm.lost_now[k] = sm.pool[sm.ut[k]];
+            // u_det1: the detections association 2 left, for association 3
+            const int nud1 = block_compact(nud0, [&](int j) { return y[j] < 0; }, sm.lo, sm.misc);
+            for (int k = tid; k < nud1; k += nthr) sm.hi[k] = sm.udets0[sm.lo[k]];
+            __syncthreads();
+            for (int k = tid; k < nud1; k += nthr) sm.udets0[k] = sm.hi[k];
+            nud0 = nud1;
+            __syncthreads();
+        } else if (sort) {
             // basetrack.py:429-433: unmatched Tracked rows become lost
             for (int k = tid; k < nut; k += nthr) { const int s = sm.pool[sm.ut[k]]; v.state[s] = ST_LOST; sm.lost_now[k] = s; }
             nlostnow = nut;
@@ -724,7 +839,12 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
             for (int q = 0; q < 4; ++q) sm.colbox[4 * k + q] = sm.detbox[4 * sm.udets0[k] + q];
         __syncthreads();
         const AppCtx app3 = {sm.unconf, sm.udets0, feats, p.theta_iou, p.theta_emb};
-        associate<T>(c, nunc, nud0, (T)p.t3, err, nullptr, nullptr, feats ? &app3 : nullptr);
+        if constexpr (SS) {
+            const DenseCtx d3 = {sm.unconf, sm.udets0, dist, st.dmax, gamma};
+            associate<T, true>(c, nunc, nud0, (T)p.t3, err, nullptr, nullptr, nullptr, &d3);
+        } else {
+            associate<T>(c, nunc, nud0, (T)p.t3, err, nullptr, nullptr, feats ? &app3 : nullptr);
+        }
         for (int k = tid; k < nunc; k += nthr)
             if (x[k] < 0) { const int s = sm.unconf[k]; v.state[s] = ST_REMOVED; if (v.removed_at[s] == 0) v.removed_at[s] = f; }
         // births (q3: BoT-SORT walks every first-stage leftover, the others only third-stage leftovers)
@@ -787,13 +907,25 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
     // ---- P9: list algebra (bytetrack.py:186-193)
     int nt1 = block_compact(n_tracked0, [&](int k) { return v.state[v.tracked[k]] == ST_TRACKED; }, sm.ut, sm.misc);
     for (int k = tid; k < nt1; k += nthr) sm.ntr[k] = v.tracked[sm.ut[k]];
+    if constexpr (SS) {
+        // joint_stracks(tracked, activated_starcks) (strongsort.py:233): an updated track that q18 marked lost left the filtered
+        // list and comes back here, in activated_starcks order -- association 1's updates, then association 2's
+        if (!p.predict_only) {
+            for (int bit = 1; bit <= 4; bit += 3) {
+                const int ne = block_compact(npool, [&](int k) { return (sm.dupa[k] & (8 | bit)) == (8 | bit); }, sm.ut, sm.misc);
+                for (int k = tid; k < ne; k += nthr) sm.ntr[nt1 + k] = sm.pool[sm.ut[k]];
+                nt1 += ne;
+            }
+        }
+    }
     for (int k = tid; k < nbirth; k += nthr) sm.ntr[nt1 + k] = sm.births[k];
     for (int k = tid; k < nref; k += nthr) sm.ntr[nt1 + nbirth + k] = sm.refind[k];
     nt1 += nbirth + nref;
     if (nt1 > cap) { nt1 = cap; if (tid == 0) *err |= ERR_SLOTS; }
     // old lost entries that were not re-found and whose id was not in the removed list before this frame
+    // (StrongSORT: "not re-found" is frame_id != f -- a re-found track that q18 marked lost is Lost again, yet on the tracked list)
     int nl1 = block_compact(n_lost0, [&](int k) { const int s = v.lost[k];
-        return v.state[s] != ST_TRACKED && !(v.removed_at[s] != 0 && v.removed_at[s] < f); }, sm.ut, sm.misc);
+        return (SS ? v.frame_id[s] != f : v.state[s] != ST_TRACKED) && !(v.removed_at[s] != 0 && v.removed_at[s] < f); }, sm.ut, sm.misc);
     for (int k = tid; k < nl1; k += nthr) sm.nlo[k] = v.lost[sm.ut[k]];
     __syncthreads();
     const int nl_add = block_compact(nlostnow, [&](int k) { const int s = sm.lost_now[k];

@@ -5,6 +5,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <cstddef>
 #include "b2t_step.cuh"
 #include "../../include/b200track.h"
 
@@ -30,7 +31,7 @@ static int check_launch(const char* what) {
     return B2T_OK;
 }
 extern "C" const char* b2t_last_error(void) { return g_err.c_str(); }
-extern "C" int b2t_version(void) { return 104; }
+extern "C" int b2t_version(void) { return 105; }
 extern "C" long long b2t_launch_count(void) { return g_launches; }
 
 // ------------------------------------------------------------------------------------------ Kalman kernels
@@ -220,6 +221,93 @@ __global__ void lap_solve_kernel(int n, int m, T thresh, const int* e_col, const
     for (int j = (int)threadIdx.x; j < m; j += (int)blockDim.x) y[(size_t)batch * m + j] = w.y[j];
 }
 
+// ------------------------------------------------------------------------------------------ feature distances
+// StrongSORT's appearance cost, matching.embedding_distance(metric='euclidean') (matching.py:95-98): out[s][row][j] = |a_row - b_j|
+// in float64 for float32 feature rows, max(0, .) as the reference clamps it.
+// One CTA of 256 threads per 64 x 64 tile of (row, column) pairs; K is staged through shared memory FD_K floats at a time, and each
+// thread keeps a 4 x 4 register block of sums ((double)a - (double)b)^2, accumulated in k order (separate multiply and add, the unit
+// is built with --fmad=false).  The difference form keeps identical rows at exactly 0.  Each float32 input is exact in float64, so
+// the error is that of D subtractions, D squares, D - 1 additions and the square root: |out - exact| <= gamma_{D+3} * exact, with
+// gamma_k = k u / (1 - k u), u = 2^-53 (tests/featdist_ref.py).
+// Rows: with ctrl (the fused step), the sequence's tracked list followed by its lost list, read at frame start; the row is written at
+// out row = slot.  Without ctrl, rows 0..n-1.  Columns: 0..min(det_count[s], m)-1, or 0..m-1 without det_count.  A tile beyond the
+// rows or columns in use returns at once.  The grid is linear: S x tiles_r x tiles_c CTAs.
+constexpr int FD_T = 64, FD_K = 16;
+__global__ void __launch_bounds__(256)
+feat_dist_kernel(const float* a, size_t a_seq, const float* b, size_t b_seq, int D, int n, int m, const int* ctrl, const int* tracked,
+                 const int* lost, int cap, const int* det_count, double* out, size_t out_seq, int ld, int tiles_r, int tiles_c) {
+    __shared__ float As[FD_T][FD_K + 1];
+    __shared__ float Bs[FD_T][FD_K + 1];
+    __shared__ int rslot[FD_T];
+    const int tile = (int)blockIdx.x, per_seq = tiles_r * tiles_c;
+    const int s = tile / per_seq, tr = (tile % per_seq) / tiles_c, tc = tile % tiles_c;
+    const int nt = ctrl ? ctrl[(size_t)s * 16 + CTRL_NTRACKED] : n;
+    const int nrows = ctrl ? nt + ctrl[(size_t)s * 16 + CTRL_NLOST] : n;
+    int ncols = m;
+    if (det_count && det_count[s] < m) ncols = det_count[s];
+    const int r0 = tr * FD_T, c0 = tc * FD_T;
+    if (r0 >= nrows || c0 >= ncols) return;
+    const int tid = (int)threadIdx.x;
+    if (tid < FD_T) {
+        const int r = r0 + tid;
+        int slot = -1;
+        if (r < nrows) slot = !ctrl ? r : r < nt ? tracked[(size_t)s * cap + r] : lost[(size_t)s * cap + r - nt];
+        rslot[tid] = slot;
+    }
+    __syncthreads();
+    const float* as = a + (size_t)s * a_seq;
+    const float* bs = b + (size_t)s * b_seq;
+    const int tx = tid & 15, ty = tid >> 4;
+    double acc[4][4];
+    for (int i = 0; i < 4; ++i)
+        for (int j = 0; j < 4; ++j) acc[i][j] = 0.0;
+    for (int k0 = 0; k0 < D; k0 += FD_K) {
+        for (int q = tid; q < FD_T * FD_K; q += 256) {
+            const int rr = q / FD_K, kk = q % FD_K, k = k0 + kk, sl = rslot[rr], cj = c0 + rr;
+            As[rr][kk] = (sl >= 0 && k < D) ? as[(size_t)sl * D + k] : 0.f;      // zero padding adds exact zeros
+            Bs[rr][kk] = (cj < ncols && k < D) ? bs[(size_t)cj * D + k] : 0.f;
+        }
+        __syncthreads();
+#pragma unroll 4
+        for (int kk = 0; kk < FD_K; ++kk) {
+            double av[4], bv[4];
+            for (int i = 0; i < 4; ++i) av[i] = (double)As[ty + 16 * i][kk];
+            for (int j = 0; j < 4; ++j) bv[j] = (double)Bs[tx + 16 * j][kk];
+            for (int i = 0; i < 4; ++i)
+                for (int j = 0; j < 4; ++j) { const double d = av[i] - bv[j]; acc[i][j] = acc[i][j] + d * d; }
+        }
+        __syncthreads();
+    }
+    double* os = out + (size_t)s * out_seq;
+    for (int i = 0; i < 4; ++i) {
+        const int sl = rslot[ty + 16 * i];
+        if (sl < 0) continue;
+        for (int j = 0; j < 4; ++j) {
+            const int cj = c0 + tx + 16 * j;
+            if (cj < ncols) os[(size_t)sl * ld + cj] = sqrt(fmax(0.0, acc[i][j]));
+        }
+    }
+}
+
+static int feat_dist_launch(const float* a, size_t a_seq, const float* b, size_t b_seq, int D, int n, int m, const int* ctrl,
+                            const int* tracked, const int* lost, int cap, const int* det_count, double* out, size_t out_seq, int ld,
+                            int batch, cudaStream_t s) {
+    const int tr = (n + FD_T - 1) / FD_T, tc = (m + FD_T - 1) / FD_T;
+    B2T_LAUNCH(feat_dist_kernel, batch * tr * tc, 256, 0, s, a, a_seq, b, b_seq, D, n, m, ctrl, tracked, lost, cap, det_count, out,
+               out_seq, ld, tr, tc);
+    return check_launch("feat_dist");
+}
+
+extern "C" int b2t_feature_distance(const float* a, int n, const float* b, int m, int feat_dim, double* out, int batch, void* stream) {
+    if (n < 0 || m < 0 || batch < 0 || feat_dim < 1 || (n && m && batch && (!a || !b || !out)))
+        return fail(B2T_EINVAL, "b2t_feature_distance: bad arguments");
+    if (n == 0 || m == 0 || batch == 0) return B2T_OK;
+    if ((double)batch * ((n + FD_T - 1) / FD_T) * ((m + FD_T - 1) / FD_T) > 2147483647.0)
+        return fail(B2T_EINVAL, "b2t_feature_distance: too many tiles for one launch");
+    return feat_dist_launch(a, (size_t)n * feat_dim, b, (size_t)m * feat_dim, feat_dim, n, m, nullptr, nullptr, nullptr, 0, nullptr,
+                            out, (size_t)n * m, m, batch, (cudaStream_t)stream);
+}
+
 // ------------------------------------------------------------------------------------------ fused step
 template <class T, bool APP>
 __global__ void __launch_bounds__(512, 1)
@@ -227,6 +315,16 @@ track_step_kernel(TrackState st, StepParams prm, const float* dets, const int* d
                   const int* id_base, double* out, int out_rows, int* stat) {
     B2T_DYN_SMEM(smem_raw);
     track_step_cta<T, APP>(st, prm, (int)blockIdx.x, dets, det_count, feats, warps, id_base, out, out_rows, stat, smem_raw);
+}
+
+// StrongSORT (B2T_STRONGSORT): its own kernel, so that the instantiations above stay as they were
+template <class T>
+__global__ void __launch_bounds__(512, 1)
+track_step_ss_kernel(TrackState st, StepParams prm, const float* dets, const int* det_count, const float* feats, const double* warps,
+                     const int* id_base, double* out, int out_rows, int* stat, const double* dist, double gamma) {
+    B2T_DYN_SMEM(smem_raw);
+    track_step_cta<T, true, true>(st, prm, (int)blockIdx.x, dets, det_count, feats, warps, id_base, out, out_rows, stat, smem_raw,
+                                  dist, gamma);
 }
 
 __global__ void track_reset_kernel(TrackState st) {
@@ -414,6 +512,7 @@ struct b2t_tracker {
     size_t smem;
     // device staging for the *_host entry point (inside the state block)
     float* d_dets; int* d_count; double* d_warps; int* d_idbase; double* d_out; int* d_stat; double* d_slot; double* d_list;
+    double* dist;   // B2T_STRONGSORT: [S][cap][dmax] feature distances of the current frame
     size_t out_rows_cap;
 };
 
@@ -446,22 +545,28 @@ static void layout(const b2t_tracker_config& c, unsigned char* base, b2t_tracker
         TAKE(st.feat, float, S * cap * (size_t)c.feat_dim);
         TAKE(st.e_app, int, S * (size_t)c.ecap);
     }
+    if (c.kind == B2T_STRONGSORT) { TAKE(dist, double, S * cap * (size_t)c.dmax); }
 #undef TAKE
     *total = align_up(L.off, 256);
 }
 
 static int check_cfg(const b2t_tracker_config* c) {
     if (!c) return fail(B2T_EINVAL, "null config");
-    if (c->kind < 0 || c->kind > 2 || c->fmt < 0 || c->fmt > 2 || (c->dtype != B2T_F32 && c->dtype != B2T_F64))
+    if (c->kind < 0 || c->kind > 3 || c->fmt < 0 || c->fmt > 2 || (c->dtype != B2T_F32 && c->dtype != B2T_F64))
         return fail(B2T_EINVAL, "b2t_tracker: bad kind / fmt / dtype");
     if (c->n_seq < 1 || c->cap < 64 || c->dmax < 1 || c->dmax > 1024 || c->cap > 4096 || c->ecap < 1)
         return fail(B2T_EINVAL, "b2t_tracker: bad n_seq / cap (64..4096) / dmax (1..1024) / ecap");
+    if (c->kind == B2T_STRONGSORT) {
+        if (c->feat_dim <= 0) return fail(B2T_EINVAL, "b2t_tracker: B2T_STRONGSORT needs appearance features (feat_dim > 0)");
+        if (!(c->gamma >= 0.0 && c->gamma <= 1.0)) return fail(B2T_EINVAL, "b2t_tracker: gamma must lie in [0, 1]");
+    }
     if (c->feat_dim != 0) {
-        if (c->kind != B2T_BOTSORT) return fail(B2T_EINVAL, "b2t_tracker: feat_dim > 0 (appearance features) is only built for B2T_BOTSORT");
+        if (c->kind != B2T_BOTSORT && c->kind != B2T_STRONGSORT)
+            return fail(B2T_EINVAL, "b2t_tracker: feat_dim > 0 (appearance features) is only built for B2T_BOTSORT and B2T_STRONGSORT");
         if (c->feat_dim < 0 || c->feat_dim % 32 != 0 || c->feat_dim > 2048)
             return fail(B2T_EINVAL, "b2t_tracker: feat_dim must be 0 or a multiple of 32 up to 2048");
         // theta_iou < 1 keeps every pair with an appearance cost among the overlapping ones (the sparse candidate set)
-        if (!(c->theta_iou < 1.0) || c->theta_emb != c->theta_emb)
+        if (c->kind == B2T_BOTSORT && (!(c->theta_iou < 1.0) || c->theta_emb != c->theta_emb))
             return fail(B2T_EINVAL, "b2t_tracker: theta_iou must be < 1 and theta_emb a number");
     }
     const size_t smem = c->dtype == B2T_F64 ? StepSmem<double>::bytes(c->cap, c->dmax, 0) : StepSmem<float>::bytes(c->cap, c->dmax, 0);
@@ -487,7 +592,9 @@ extern "C" int b2t_tracker_create(const b2t_tracker_config* cfg, void* state_mem
     if (rc) return rc;
     if (!state_mem || !out || ((size_t)state_mem & 255)) return fail(B2T_EINVAL, "b2t_tracker_create: state_mem must be 256-B aligned");
     b2t_tracker* t = new b2t_tracker();
-    t->cfg = *cfg;
+    // gamma is read only for B2T_STRONGSORT: a caller built against a header without it passes a shorter struct
+    memcpy(&t->cfg, cfg, offsetof(b2t_tracker_config, gamma));
+    t->cfg.gamma = cfg->kind == B2T_STRONGSORT ? cfg->gamma : 0.0;
     size_t total;
     layout(*cfg, (unsigned char*)state_mem, t, &total);
     t->st.n_seq = cfg->n_seq; t->st.cap = cfg->cap; t->st.dmax = cfg->dmax; t->st.ecap = cfg->ecap; t->st.feat_dim = cfg->feat_dim;
@@ -502,6 +609,7 @@ extern "C" int b2t_tracker_create(const b2t_tracker_config* cfg, void* state_mem
     p.low_thresh = (float)((cfg->conf_thresh - 0.3) > 0.15 ? (cfg->conf_thresh - 0.3) : 0.15);  // bytetrack.py:15
     p.new_thresh = (float)(cfg->conf_thresh + 0.1);                                           // bytetrack.py:175
     if (cfg->kind == B2T_SORT) { p.t1 = cfg->iou_thresh; p.t2 = 0.0; p.t3 = cfg->iou_thresh + 0.1; }   // basetrack.py:414,438
+    else if (cfg->kind == B2T_STRONGSORT) { p.t1 = 0.7; p.t2 = 0.5; p.t3 = 0.7; }           // strongsort.py:158,185,209
     else { p.t1 = 0.9; p.t2 = 0.5; p.t3 = 0.7; }                                              // bytetrack.py:118,137,160
     p.t_dup = 0.15;                                                                           // basetrack.py:565
     p.max_time_lost = (int)(cfg->frame_rate / 30.0 * cfg->track_buffer);                      // basetrack.py:355-356
@@ -510,7 +618,9 @@ extern "C" int b2t_tracker_create(const b2t_tracker_config* cfg, void* state_mem
     t->smem = cfg->dtype == B2T_F64 ? StepSmem<double>::bytes(cfg->cap, cfg->dmax, t->st.esm) : StepSmem<float>::bytes(cfg->cap, cfg->dmax, t->st.esm);
     const bool app = cfg->feat_dim > 0;
     int rs;
-    if (cfg->dtype == B2T_F64) rs = app ? B2T_SET_SMEM((track_step_kernel<double, true>), t->smem) : B2T_SET_SMEM((track_step_kernel<double, false>), t->smem);
+    if (cfg->kind == B2T_STRONGSORT)
+        rs = cfg->dtype == B2T_F64 ? B2T_SET_SMEM((track_step_ss_kernel<double>), t->smem) : B2T_SET_SMEM((track_step_ss_kernel<float>), t->smem);
+    else if (cfg->dtype == B2T_F64) rs = app ? B2T_SET_SMEM((track_step_kernel<double, true>), t->smem) : B2T_SET_SMEM((track_step_kernel<double, false>), t->smem);
     else rs = app ? B2T_SET_SMEM((track_step_kernel<float, true>), t->smem) : B2T_SET_SMEM((track_step_kernel<float, false>), t->smem);
     if (rs != 0) { delete t; return fail(B2T_ECUDA, "cannot raise dynamic shared memory"); }
     *out = t;
@@ -529,7 +639,22 @@ static int step_launch(b2t_tracker* t, const float* dets, const int* det_count, 
     p.predict_only = predict_only ? 1 : 0;
     cudaStream_t s = (cudaStream_t)stream;
     const bool app = t->cfg.feat_dim > 0;
-    if (t->cfg.dtype == B2T_F64) {
+    if (t->cfg.kind == B2T_STRONGSORT) {
+        const b2t_tracker_config& c = t->cfg;
+        if (!predict_only) {
+            const size_t D = (size_t)c.feat_dim;
+            const int rc = feat_dist_launch(t->st.feat, (size_t)c.cap * D, feats, (size_t)c.dmax * D, c.feat_dim, c.cap, c.dmax, t->st.ctrl,
+                                            t->st.tracked, t->st.lost, c.cap, det_count, t->dist, (size_t)c.cap * c.dmax, c.dmax, c.n_seq, s);
+            if (rc) return rc;
+        }
+        if (c.dtype == B2T_F64) {
+            auto k = track_step_ss_kernel<double>;
+            B2T_LAUNCH(k, c.n_seq, 512, t->smem, s, t->st, p, dets, det_count, feats, warps, id_base, out, out_rows, stat, t->dist, c.gamma);
+        } else {
+            auto k = track_step_ss_kernel<float>;
+            B2T_LAUNCH(k, c.n_seq, 512, t->smem, s, t->st, p, dets, det_count, feats, warps, id_base, out, out_rows, stat, t->dist, c.gamma);
+        }
+    } else if (t->cfg.dtype == B2T_F64) {
         auto k = app ? track_step_kernel<double, true> : track_step_kernel<double, false>;
         B2T_LAUNCH(k, t->cfg.n_seq, 512, t->smem, s, t->st, p, dets, det_count, feats, warps, id_base, out, out_rows, stat);
     } else {
