@@ -58,9 +58,10 @@ int b2t_kalman_project(int dtype, int fmt, const void* mean, const void* cov, co
 int b2t_kalman_update(int dtype, int fmt, void* mean, void* cov, const int* idx, const void* meas,
                       const float* conf, const int* flags, int k, void* stream);
 /* KalmanFilter.gating_distance :365-411 (metric 'maha' = 0, 'gaussian' = 1).  One state vs m
- * measurements: mean [8], cov [64], meas [m][4] -> out [m]. */
+ * measurements: mean [8], cov [64], meas [m][4] -> out [m].  flags: B2T_FLAG_MEAN_F32 when the caller's
+ * mean is still float32 (project then rounds the noise std to float32, as update does), else 0. */
 int b2t_kalman_gating(int dtype, int fmt, const void* mean, const void* cov, const void* meas, int m,
-                      int only_position, int metric, void* out, void* stream);
+                      int only_position, int metric, int flags, void* out, void* stream);
 /* botsort.multi_gmc, tracker/botsort.py:250-269.  warp_host: 6 doubles {a00,a01,tx,a10,a11,ty} on the HOST. */
 int b2t_gmc_apply(int dtype, void* mean, void* cov, int n, const double* warp_host, void* stream);
 

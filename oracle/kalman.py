@@ -124,9 +124,9 @@ def update(fmt, mean, cov, z, mean_f32=False, confidence=0.0):
     return new_mean, new_cov
 
 
-def gating_distance(fmt, mean, cov, measurements, only_position=False, metric="maha"):
-    """kalman_filter.py:365-411."""
-    z_hat, s = project(fmt, mean, cov)
+def gating_distance(fmt, mean, cov, measurements, only_position=False, metric="maha", mean_f32=False):
+    """kalman_filter.py:365-411.  ``mean_f32``: the mean is still float32, so project rounds the noise std to float32."""
+    z_hat, s = project(fmt, mean, cov, mean_f32)
     measurements = np.asarray(measurements, dtype=np.float64)
     if only_position:
         z_hat, s = z_hat[:2], s[:2, :2]

@@ -56,7 +56,7 @@ SIGNATURES = {
     "b2t_kalman_predict": (_I, [_I, _I, _P, _P, _P, _I, _I, _P]),
     "b2t_kalman_project": (_I, [_I, _I, _P, _P, _P, _P, _P, _P, _I, _P]),
     "b2t_kalman_update": (_I, [_I, _I, _P, _P, _P, _P, _P, _P, _I, _P]),
-    "b2t_kalman_gating": (_I, [_I, _I, _P, _P, _P, _I, _I, _I, _P, _P]),
+    "b2t_kalman_gating": (_I, [_I, _I, _P, _P, _P, _I, _I, _I, _I, _P, _P]),
     "b2t_gmc_apply": (_I, [_I, _P, _P, _I, C.POINTER(C.c_double), _P]),
     "b2t_iou_cost": (_I, [_I, _P, _I, _P, _I, _P, _I, _I, _I, _P]),
     "b2t_lap_workspace_bytes": (_SZ, [_I, _I, _I, _I]),

@@ -291,11 +291,11 @@ class Ops:
         L.check(self.lib, self.lib.b2t_kalman_update(dtype, fmt, _dev_ptr(mean), _dev_ptr(cov), _dev_ptr(idx), _dev_ptr(meas),
                                                      _dev_ptr(conf), _dev_ptr(flags), meas.shape[0], self._s()))
 
-    def kalman_gating(self, dtype, fmt, mean, cov, meas, only_position=False, metric=0):
+    def kalman_gating(self, dtype, fmt, mean, cov, meas, only_position=False, metric=0, mean_f32=False):
         m = meas.shape[0]
         out = torch.empty(m, dtype=_tdt(dtype), device=self.device)
-        L.check(self.lib, self.lib.b2t_kalman_gating(dtype, fmt, _dev_ptr(mean), _dev_ptr(cov), _dev_ptr(meas), m,
-                                                     int(only_position), int(metric), _dev_ptr(out), self._s()))
+        L.check(self.lib, self.lib.b2t_kalman_gating(dtype, fmt, _dev_ptr(mean), _dev_ptr(cov), _dev_ptr(meas), m, int(only_position),
+                                                     int(metric), L.FLAG_MEAN_F32 if mean_f32 else 0, _dev_ptr(out), self._s()))
         return out
 
     def gmc_apply(self, dtype, mean, cov, warp):

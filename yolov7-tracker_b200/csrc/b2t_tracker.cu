@@ -31,7 +31,7 @@ static int check_launch(const char* what) {
     return B2T_OK;
 }
 extern "C" const char* b2t_last_error(void) { return g_err.c_str(); }
-extern "C" int b2t_version(void) { return 105; }
+extern "C" int b2t_version(void) { return 106; }
 extern "C" long long b2t_launch_count(void) { return g_launches; }
 
 // ------------------------------------------------------------------------------------------ Kalman kernels
@@ -114,17 +114,18 @@ __global__ void kalman_project_kernel(int fmt, const T* mean, const T* cov, cons
     }
 }
 
-// gating_distance: one state, thread per measurement.
+// gating_distance: one state, thread per measurement.  mean_f32: the caller's mean is still float32, so the reference's project
+// rounds the noise std to float32 (kf_r), as update does.
 template <class T>
 __global__ void kalman_gating_kernel(int fmt, const T* mean, const T* cov, const T* meas, int m, int only_position,
-                                     int metric, T* out) {
+                                     int metric, bool mean_f32, T* out) {
     const int i = (int)(blockIdx.x * blockDim.x + threadIdx.x);
     if (i >= m) return;
     const int nd = only_position ? 2 : 4;
     T S[4][4], d[4];
     for (int a = 0; a < 4; ++a) {
         for (int b = 0; b < 4; ++b) S[a][b] = cov[a * 8 + b];
-        S[a][a] = S[a][a] + kf_r<T>(a, fmt, mean[2], mean[3], false, -1.f);
+        S[a][a] = S[a][a] + kf_r<T>(a, fmt, mean[2], mean[3], mean_f32, -1.f);
         d[a] = meas[(size_t)i * 4 + a] - mean[a];
     }
     T acc = (T)0;
@@ -423,13 +424,14 @@ extern "C" int b2t_kalman_update(int dtype, int fmt, void* mean, void* cov, cons
 }
 
 extern "C" int b2t_kalman_gating(int dtype, int fmt, const void* mean, const void* cov, const void* meas, int m,
-                                 int only_position, int metric, void* out, void* stream) {
+                                 int only_position, int metric, int flags, void* out, void* stream) {
     if (m < 0 || fmt < 0 || fmt > 2 || metric < 0 || metric > 1) return fail(B2T_EINVAL, "b2t_kalman_gating: bad arguments");
+    const bool f32 = (flags & B2T_FLAG_MEAN_F32) != 0;
     if (m == 0) return B2T_OK;
     cudaStream_t s = (cudaStream_t)stream;
     DISPATCH(dtype,
-        B2T_LAUNCH(kalman_gating_kernel<float>, (m + 127) / 128, 128, 0, s, fmt, (const float*)mean, (const float*)cov, (const float*)meas, m, only_position, metric, (float*)out),
-        B2T_LAUNCH(kalman_gating_kernel<double>, (m + 127) / 128, 128, 0, s, fmt, (const double*)mean, (const double*)cov, (const double*)meas, m, only_position, metric, (double*)out));
+        B2T_LAUNCH(kalman_gating_kernel<float>, (m + 127) / 128, 128, 0, s, fmt, (const float*)mean, (const float*)cov, (const float*)meas, m, only_position, metric, f32, (float*)out),
+        B2T_LAUNCH(kalman_gating_kernel<double>, (m + 127) / 128, 128, 0, s, fmt, (const double*)mean, (const double*)cov, (const double*)meas, m, only_position, metric, f32, (double*)out));
     return check_launch("kalman_gating");
 }
 

@@ -94,7 +94,8 @@ class _GpuKalman(object):
         m = ops.dev(np.asarray(mean, dtype=np.float64).reshape(8), torch.float64)
         c = ops.dev(np.asarray(covariance, dtype=np.float64).reshape(8, 8), torch.float64)
         z = ops.dev(np.asarray(measurements, dtype=np.float64).reshape(-1, 4), torch.float64)
-        return ops.kalman_gating(L.F64, self._fmt, m, c, z, only_position, 0 if metric == 'maha' else 1).cpu().numpy()
+        return ops.kalman_gating(L.F64, self._fmt, m, c, z, only_position, 0 if metric == 'maha' else 1,
+                                 _flags_for(mean) != 0).cpu().numpy()
 
 
 class KalmanFilter(_GpuKalman):
