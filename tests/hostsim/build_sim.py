@@ -36,12 +36,13 @@ def build(force=False):
     return LIB
 
 
-def build_variant(name, patches):
-    """A simulator build of the tracker translation unit with source edits (a test's injected bug): patches = [(file, old, new)],
-    each `old` found exactly once.  Built in a temporary directory; returns the library's path."""
+def build_variant(name, patches, units=("b2t_tracker.cu",)):
+    """A simulator build of translation units `units` (csrc file names; the tracker's by default) with source edits (a test's
+    injected bug): patches = [(file, old, new)], each `old` found exactly once.  Built in a temporary directory; returns the
+    library's path."""
     import shutil
     import tempfile
-    h = hashlib.sha1((_digest() + repr(patches)).encode()).hexdigest()[:16]
+    h = hashlib.sha1((_digest() + repr(patches) + repr(tuple(units))).encode()).hexdigest()[:16]
     out = os.path.join(tempfile.gettempdir(), "b2t_hostsim_variants_%d" % os.getuid(), "%s_%s" % (name, h))
     lib = os.path.join(out, "lib.so")
     if os.path.exists(lib):
@@ -55,8 +56,10 @@ def build_variant(name, patches):
         s = open(p).read()
         assert s.count(old) == 1, "patch for %s: %r found %d times" % (fn, old, s.count(old))
         open(p, "w").write(s.replace(old, new))
-    cmd = ["g++", "-O1", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-DB2T_HOSTSIM", "-I", HERE, "-I", src,
-           "-x", "c++", os.path.join(src, "b2t_tracker.cu"), "-x", "c++", os.path.join(HERE, "cuda_sim.cpp"), "-o", lib + ".tmp"]
+    cmd = ["g++", "-O1", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-DB2T_HOSTSIM", "-I", HERE, "-I", src]
+    for u in units:
+        cmd += ["-x", "c++", os.path.join(src, u)]
+    cmd += ["-x", "c++", os.path.join(HERE, "cuda_sim.cpp"), "-o", lib + ".tmp"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("hostsim variant build failed:\n" + r.stderr[-6000:])
