@@ -76,6 +76,33 @@ int b2t_iou_cost(int dtype, const void* a, int n, const void* b, int m, void* co
 size_t b2t_lap_workspace_bytes(int dtype, int n, int m, int batch);
 int b2t_lap_solve(int dtype, const void* cost, int n, int m, int ld, double thresh, int* x, int* y,
                   void* workspace, size_t workspace_bytes, int batch, void* stream);
+/* The same solver on a caller-given contiguous CSR, stored the way the fused tracker step stores its
+ * associations -- for checking each storage path of the solver directly.  Problem b of the batch (one CTA):
+ *   rows [row_off, row_off + n) of row_start / row_cnt (row_start relative to entry_off), its result in
+ *   x[row_off ..] and y[col_off ..]; entries [entry_off, entry_off + n_entries) of e_col / e_cost / e_row
+ *   (col -1 = padding, only entries with cost < thresh may be listed);
+ *   entries [0, s_cap) of the mirror arrays m_* are copied into shared memory, and a row ending at or
+ *   below s_cap is read there; [w2_base, w2_end) of m_* is copied into a second shared-memory window, read for
+ *   the rows inside it (a row may straddle w2_end).  m_col = m_cost = NULL: the mirrors are copies of e_*.
+ *   rowwise != 0 hands the solver no row index (e_row = NULL, n_entries = 0), as the step does when its
+ *   edges overflow: row-parallel kernelisation and labelling instead of the edge-parallel forms.  Row
+ *   indices (e_row, and m_row when the mirrors are given) are read only for problems with rowwise = 0,
+ *   and may be NULL when every problem is row-parallel; B2T_EINVAL otherwise.
+ * counters [batch][B2T_LAP_COUNTERS]: kernelisation rounds, rows left after kernelisation, searches retried
+ * on one warp after outgrowing their warp's 64-column frontier.  B2T_ECAPACITY, with nothing launched, when
+ * the largest n, m and windows of the batch need more than 227 KB of shared memory.
+ * workspace: b2t_lap_csr_workspace_bytes(batch) bytes of device memory. */
+enum { B2T_LAP_COUNTERS = 3 };
+typedef struct b2t_lap_csr_problem {
+    int n, m;
+    double thresh;
+    int row_off, col_off, entry_off, n_entries;
+    int s_cap, w2_base, w2_end, rowwise;
+} b2t_lap_csr_problem;
+size_t b2t_lap_csr_workspace_bytes(int batch);
+int b2t_lap_solve_csr(int dtype, const b2t_lap_csr_problem* probs_host, int batch, const int* row_start, const int* row_cnt,
+                      const int* e_col, const void* e_cost, const int* e_row, const int* m_col, const void* m_cost,
+                      const int* m_row, int* x, int* y, int* counters, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------- fused trackers
  * One object = S independent video sequences advanced together, one CTA per sequence per frame:

@@ -37,6 +37,17 @@ class TrackerConfig(C.Structure):
                 ("feat_dim", C.c_int), ("theta_iou", C.c_double), ("theta_emb", C.c_double), ("gamma", C.c_double)]
 
 
+class LapCsrProblem(C.Structure):
+    """b2t_lap_csr_problem: one problem of b2t_lap_solve_csr."""
+    _fields_ = [("n", C.c_int), ("m", C.c_int), ("thresh", C.c_double), ("row_off", C.c_int), ("col_off", C.c_int),
+                ("entry_off", C.c_int), ("n_entries", C.c_int), ("s_cap", C.c_int), ("w2_base", C.c_int), ("w2_end", C.c_int),
+                ("rowwise", C.c_int)]
+
+
+LAP_COUNTERS = 3          # kernelisation rounds, rows left after kernelisation, frontier-overflow retries
+EINVAL, ECAPACITY = -1, -3
+
+
 class ConvDesc(C.Structure):
     _fields_ = [("x", C.c_void_p), ("w_packed", C.c_void_p), ("bias", C.c_void_p), ("y", C.c_void_p),
                 ("n", C.c_int), ("h", C.c_int), ("w", C.c_int), ("cin", C.c_int), ("in_pitch", C.c_int), ("in_coff", C.c_int),
@@ -61,6 +72,8 @@ SIGNATURES = {
     "b2t_iou_cost": (_I, [_I, _P, _I, _P, _I, _P, _I, _I, _I, _P]),
     "b2t_lap_workspace_bytes": (_SZ, [_I, _I, _I, _I]),
     "b2t_lap_solve": (_I, [_I, _P, _I, _I, _I, _D, _P, _P, _P, _SZ, _I, _P]),
+    "b2t_lap_csr_workspace_bytes": (_SZ, [_I]),
+    "b2t_lap_solve_csr": (_I, [_I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _SZ, _P]),
     "b2t_tracker_state_bytes": (_SZ, [C.POINTER(TrackerConfig)]),
     "b2t_tracker_create": (_I, [C.POINTER(TrackerConfig), _P, _P, C.POINTER(_P)]),
     "b2t_tracker_reset": (_I, [_P, _P]),

@@ -251,18 +251,32 @@ B2T_DEV bool lap_augment_row(const LapCsr<T>& g, const T half_t, LapWork<T>& w, 
 }
 
 // Kernelisation keys: the weight rounded to float32, as an order-preserving unsigned (weights are
-// positive).  Shared-memory atomicMax is native for 32 bits (the 64-bit form is a CAS loop).  The
-// float rounding (<= 6e-8 relative) is absorbed by the rule's margin, see lap_kernelize_*.
+// positive).  Shared-memory atomicMax is native for 32 bits (the 64-bit form is a CAS loop).
 B2T_DEV unsigned int wkey32(float v) { unsigned int k; memcpy(&k, &v, 4); return k; }
 B2T_DEV float wval32(unsigned int k) { float v; memcpy(&v, &k, 4); return v; }
-#define B2T_KMARGIN 2e-6f
+// The key of a live edge (weight t - c > 0): at least 1, so that key 0 always means "no edge" -- a
+// float64 weight below half of float32's smallest denormal would otherwise round to key 0 and its row
+// would be dropped as edgeless.  The clamp is monotone, so the order of the keys is kept.
+template <class T> B2T_DEV unsigned int wkey_live(T w) { const unsigned int k = wkey32((float)w); return k ? k : 1u; }
+// An upper bound of every weight whose key is k: the next float up.  Rounding to nearest can put
+// the key up to half a float ulp BELOW the weight (at weights >= 32 that is more than 2e-6), but
+// the next float lies strictly above it.  Key 0 (no edge) gives the smallest denormal; the key of
+// +inf (a weight beyond float range) gives NaN, and a comparison with NaN never fixes an edge.
+B2T_DEV double wup32(unsigned int k) { return (double)wval32(k + 1u); }
 
-// Exact kernelisation, row-parallel form (any CSR).  A mutually-best edge (i, j) is fixed when
-//      w_ij > second_best(i) + second_best(j) + margin.
-// Column-side best / second-best are reduced with 32-bit shared-memory atomics on float keys (ties
-// for a column's best go to the smallest row; a tie makes second-best == best so the rule cannot
-// fire).  The keys only ever make the test MORE conservative: a fixed edge is always a true
-// strictly dominant one, so exactness is preserved.  All threads; leaves w.rdead / w.cdead / x / y.
+// Exact kernelisation, row-parallel form (any CSR).  An edge (i, j) whose weight W exceeds S_i + S_j,
+// where S_i / S_j bound the weight of every OTHER live edge at row i / column j, belongs to every
+// optimal matching: a matching without it loses at most S_i + S_j by dropping the edges at i and j
+// and gains W by taking (i, j).  The rule fixes a mutually-best edge when
+//      (double)t - (double)c_ij  >  wup32(second key at i) + wup32(second key at j)
+// in float64, in both instantiations.  Each wup32 lies strictly above its true second best, so
+// U = wup32 + wup32 > S_i + S_j exactly.  Each side of the test is ONE rounding of an exact value
+// (W = t - c of two floats or two doubles, U of two floats), and rounding is monotone: W <= U
+// implies fl(W) <= fl(U).  So a fired test implies W > U > S_i + S_j for any finite weight, with no
+// absolute margin.  (The argument holds in float32 arithmetic too; evaluating in float64 makes both
+// instantiations take the same decision on a problem whose costs are float32.)  Column-side best / second-best are reduced with 32-bit shared-memory atomics on
+// the keys (ties for a column's best go to the smallest row, and the other rows of the tie then set
+// the second key to the best key, so the rule cannot fire).  All threads; leaves w.rdead / w.cdead / x / y.
 template <class T>
 B2T_DEVNI void lap_kernelize_rows(int n, int m, const LapCsr<T>& g, T thresh, LapWork<T>& w) {
     const int tid = (int)threadIdx.x, nthr = (int)blockDim.x;
@@ -278,7 +292,7 @@ B2T_DEVNI void lap_kernelize_rows(int n, int m, const LapCsr<T>& g, T thresh, La
             const int es = g.start(i), ec = g.row_cnt[i];
             const int* ecol = g.cols(es, ec);
             const T* ecost = g.costs(es, ec);
-            for (int e = 0; e < ec; ++e) { const int j = ecol[e]; if (j >= 0 && !w.cdead[j]) atomicMax(&cb[j], wkey32((float)(thresh - ecost[e]))); }
+            for (int e = 0; e < ec; ++e) { const int j = ecol[e]; if (j >= 0 && !w.cdead[j]) atomicMax(&cb[j], wkey_live<T>(thresh - ecost[e])); }
         }
         __syncthreads();
         for (int i = tid; i < n; i += nthr) {
@@ -286,7 +300,7 @@ B2T_DEVNI void lap_kernelize_rows(int n, int m, const LapCsr<T>& g, T thresh, La
             const int es = g.start(i), ec = g.row_cnt[i];
             const int* ecol = g.cols(es, ec);
             const T* ecost = g.costs(es, ec);
-            for (int e = 0; e < ec; ++e) { const int j = ecol[e]; if (j >= 0 && !w.cdead[j] && wkey32((float)(thresh - ecost[e])) == cb[j]) atomicMin(&cbrow[j], i); }
+            for (int e = 0; e < ec; ++e) { const int j = ecol[e]; if (j >= 0 && !w.cdead[j] && wkey_live<T>(thresh - ecost[e]) == cb[j]) atomicMin(&cbrow[j], i); }
         }
         __syncthreads();
         for (int i = tid; i < n; i += nthr) {
@@ -294,7 +308,7 @@ B2T_DEVNI void lap_kernelize_rows(int n, int m, const LapCsr<T>& g, T thresh, La
             const int es = g.start(i), ec = g.row_cnt[i];
             const int* ecol = g.cols(es, ec);
             const T* ecost = g.costs(es, ec);
-            for (int e = 0; e < ec; ++e) { const int j = ecol[e]; if (j >= 0 && !w.cdead[j] && cbrow[j] != i) atomicMax(&cs[j], wkey32((float)(thresh - ecost[e]))); }
+            for (int e = 0; e < ec; ++e) { const int j = ecol[e]; if (j >= 0 && !w.cdead[j] && cbrow[j] != i) atomicMax(&cs[j], wkey_live<T>(thresh - ecost[e])); }
         }
         __syncthreads();
         for (int i = tid; i < n; i += nthr) {
@@ -302,20 +316,24 @@ B2T_DEVNI void lap_kernelize_rows(int n, int m, const LapCsr<T>& g, T thresh, La
             const int es = g.start(i), ec = g.row_cnt[i];
             const int* ecol = g.cols(es, ec);
             const T* ecost = g.costs(es, ec);
-            T w1 = (T)0, w2 = (T)0;
+            T w1 = (T)0, w2 = (T)0, c1 = (T)0;
             int j1 = -1;
             for (int e = 0; e < ec; ++e) {
                 const int j = ecol[e];
                 if (j < 0 || w.cdead[j]) continue;
                 const T ww = thresh - ecost[e];
-                if (ww > w1) { w2 = w1; w1 = ww; j1 = j; } else if (ww > w2) w2 = ww;
+                if (ww > w1) { w2 = w1; w1 = ww; j1 = j; c1 = ecost[e]; } else if (ww > w2) w2 = ww;
             }
             if (j1 < 0) { w.rdead[i] = 1; continue; }                          // no live edge left: stays unmatched
-            if (cbrow[j1] == i && w1 > w2 + (T)wval32(cs[j1]) + (T)B2T_KMARGIN) {
-                w.x[i] = j1; w.y[j1] = i; w.rdead[i] = 1; w.cdead[j1] = 1; w.scratch[44] = 1;
+            // (the row's second best through its key as well: in float32, t - c may have rounded below its true weight)
+            if (cbrow[j1] == i && (double)thresh - (double)c1 > wup32(wkey32((float)w2)) + wup32(cs[j1])) {
+                w.x[i] = j1; w.y[j1] = i; w.scratch[44] = 1; w.sc[j1] = 2;
             }
         }
         __syncthreads();
+        // retire the fixed pairs in a separate pass: a row testing the rule must not see a column another row fixed in the same
+        // pass, or how far a chain of fixes runs in one round would depend on thread timing
+        for (int j = tid; j < m; j += nthr) if (w.sc[j] == 2) { w.sc[j] = 0; w.cdead[j] = 1; w.rdead[w.y[j]] = 1; }
         const int changed = w.scratch[44];
         if (tid == 0) w.scratch[46] = round + 1;
         __syncthreads();
@@ -344,14 +362,14 @@ B2T_DEVNI void lap_kernelize_edges(int n, int m, const LapCsr<T>& g, T thresh, L
         for (int e = tid; e < nE; e += nthr) {
             int i, j; T c;
             if (!g.entry(e, n, i, j, c) || j < 0 || w.rdead[i] || w.cdead[j]) continue;
-            const unsigned k = wkey32((float)(thresh - c));
+            const unsigned k = wkey_live<T>(thresh - c);
             atomicMax(&cb[j], k); atomicMax(&rb[i], k);
         }
         __syncthreads();
         for (int e = tid; e < nE; e += nthr) {
             int i, j; T c;
             if (!g.entry(e, n, i, j, c) || j < 0 || w.rdead[i] || w.cdead[j]) continue;
-            const unsigned k = wkey32((float)(thresh - c));
+            const unsigned k = wkey_live<T>(thresh - c);
             if (k == cb[j]) atomicMin(&cbrow[j], i);
             if (k == rb[i]) atomicMin(&rbcol[i], j);
         }
@@ -359,7 +377,7 @@ B2T_DEVNI void lap_kernelize_edges(int n, int m, const LapCsr<T>& g, T thresh, L
         for (int e = tid; e < nE; e += nthr) {
             int i, j; T c;
             if (!g.entry(e, n, i, j, c) || j < 0 || w.rdead[i] || w.cdead[j]) continue;
-            const unsigned k = wkey32((float)(thresh - c));
+            const unsigned k = wkey_live<T>(thresh - c);
             if (cbrow[j] != i) atomicMax(&cs[j], k);
             if (rbcol[i] != j) atomicMax(&rs[i], k);
         }
@@ -368,10 +386,9 @@ B2T_DEVNI void lap_kernelize_edges(int n, int m, const LapCsr<T>& g, T thresh, L
         for (int e = tid; e < nE; e += nthr) {
             int i, j; T c;
             if (!g.entry(e, n, i, j, c) || j < 0 || w.rdead[i] || w.cdead[j]) continue;
-            if (cbrow[j] == i && rbcol[i] == j) {
-                const T w1 = thresh - c;
-                // guard against two float-tied edges of the same (i, j) pair of lists: the pair (i, j) is unique per row
-                if (w1 > (T)wval32(rs[i]) + (T)wval32(cs[j]) + (T)B2T_KMARGIN) { w.x[i] = j; w.y[j] = i; w.scratch[44] = 1; w.sc[j] = 2; }
+            // the rule of lap_kernelize_rows, with both second bests from keys
+            if (cbrow[j] == i && rbcol[i] == j && (double)thresh - (double)c > wup32(rs[i]) + wup32(cs[j])) {
+                w.x[i] = j; w.y[j] = i; w.scratch[44] = 1; w.sc[j] = 2;
             }
         }
         __syncthreads();

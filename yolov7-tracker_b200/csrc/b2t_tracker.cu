@@ -31,7 +31,7 @@ static int check_launch(const char* what) {
     return B2T_OK;
 }
 extern "C" const char* b2t_last_error(void) { return g_err.c_str(); }
-extern "C" int b2t_version(void) { return 106; }
+extern "C" int b2t_version(void) { return 107; }
 extern "C" long long b2t_launch_count(void) { return g_launches; }
 
 // ------------------------------------------------------------------------------------------ Kalman kernels
@@ -220,6 +220,48 @@ __global__ void lap_solve_kernel(int n, int m, T thresh, const int* e_col, const
     lap_solve_cta<T>(n, m, g, thresh, w);
     for (int i = (int)threadIdx.x; i < n; i += (int)blockDim.x) x[(size_t)batch * n + i] = w.x[i];
     for (int j = (int)threadIdx.x; j < m; j += (int)blockDim.x) y[(size_t)batch * m + j] = w.y[j];
+}
+
+// b2t_lap_solve_csr: one problem per CTA, in the LapCsr shapes step_csr builds.  Entries [0, s_cap) of the mirror arrays m_* are
+// copied into shared memory (the step's se_* storage) and [w2_base, w2_base + w2cap) into the second window; the window buffer is
+// longer than any window, as the step's is, and a reader that runs past w2_end finds whatever the caller put in m_* there.
+template <class T>
+__global__ void lap_solve_csr_kernel(const b2t_lap_csr_problem* probs, const int* row_start, const int* row_cnt, const int* e_col,
+                                     const T* e_cost, const int* e_row, const int* m_col, const T* m_cost, const int* m_row,
+                                     int nmax, int mmax, int smax, int w2cap, int* x, int* y, int* counters) {
+    B2T_DYN_SMEM(smem_raw);
+    Arena arena(smem_raw);
+    LapWork<T> w;
+    w.carve(arena, nmax, mmax);
+    int* s_col = arena.take<int>(smax); int* s_row = arena.take<int>(smax); T* s_cost = arena.take<T>(smax);
+    int* w2_col = arena.take<int>(w2cap); int* w2_row = arena.take<int>(w2cap); T* w2_cost = arena.take<T>(w2cap);
+    const b2t_lap_csr_problem p = probs[blockIdx.x];
+    const int tid = (int)threadIdx.x, nthr = (int)blockDim.x;
+    const size_t eo = (size_t)p.entry_off;
+    // (the row indices are read only by the edge-parallel passes: a row-parallel problem may come without them)
+    const bool rows = !p.rowwise;
+    for (int e = tid; e < p.s_cap; e += nthr) { s_col[e] = m_col[eo + e]; s_row[e] = rows ? m_row[eo + e] : -1; s_cost[e] = m_cost[eo + e]; }
+    const bool win = p.w2_end > p.w2_base;
+    if (win)
+        for (int k = tid; k < w2cap; k += nthr) {
+            const int e = p.w2_base + k;
+            const bool in = e < p.n_entries;
+            w2_col[k] = in ? m_col[eo + e] : -1; w2_row[k] = in && rows ? m_row[eo + e] : -1; w2_cost[k] = in ? m_cost[eo + e] : (T)0;
+        }
+    __syncthreads();
+    LapCsr<T> g;
+    g.row_start = row_start + p.row_off; g.row_stride = 0; g.row_cnt = row_cnt + p.row_off;
+    g.e_col = e_col + eo; g.e_cost = e_cost + eo;
+    g.s_col = s_col; g.s_cost = s_cost; g.s_cap = p.s_cap;
+    g.e_row = p.rowwise ? nullptr : e_row + eo; g.s_row = s_row; g.n_entries = p.rowwise ? 0 : p.n_entries;
+    if (win) { g.w2_col = w2_col; g.w2_cost = w2_cost; g.w2_row = w2_row; g.w2_base = p.w2_base; g.w2_end = p.w2_end; }
+    lap_solve_cta<T>(p.n, p.m, g, (T)p.thresh, w);
+    for (int i = tid; i < p.n; i += nthr) x[(size_t)p.row_off + i] = w.x[i];
+    for (int j = tid; j < p.m; j += nthr) y[(size_t)p.col_off + j] = w.y[j];
+    if (tid == 0) {
+        int* c = counters + (size_t)blockIdx.x * B2T_LAP_COUNTERS;
+        c[0] = w.scratch[46]; c[1] = w.scratch[45]; c[2] = w.scratch[41];
+    }
 }
 
 // ------------------------------------------------------------------------------------------ feature distances
@@ -474,16 +516,16 @@ static int lap_solve_t(const T* cost, int n, int m, int ld, double thresh, int* 
     T* e_cost = (T*)p;            p += sizeof(T) * se * batch;
     int* e_col = (int*)p;         p += sizeof(int) * se * batch;
     int* row_cnt = (int*)p;
+    ArenaSize as;
+    LapWork<T>::size(as, n, m);
+    const size_t smem = as.off + 16;
+    if (smem > 227 * 1024) return fail(B2T_ECAPACITY, "b2t_lap_solve: n, m too large for one CTA's shared memory");   // (nothing launched)
     const int wpb = 8;
     dim3 g1((n + wpb - 1) / wpb, batch);
     auto k1 = lap_sparsify_kernel<T>;
     B2T_LAUNCH(k1, g1, wpb * 32, 0, s, cost, n, m, ld, (T)thresh, e_col, e_cost, row_cnt, se, sr);
     int rc = check_launch("lap_sparsify");
     if (rc) return rc;
-    ArenaSize as;
-    LapWork<T>::size(as, n, m);
-    const size_t smem = as.off + 16;
-    if (smem > 227 * 1024) return fail(B2T_ECAPACITY, "b2t_lap_solve: n, m too large for one CTA's shared memory");
     auto k2 = lap_solve_kernel<T>;
     if (B2T_SET_SMEM(k2, smem) != 0) return fail(B2T_ECUDA, "b2t_lap_solve: cannot raise dynamic shared memory");
     B2T_LAUNCH(k2, batch, 512, smem, s, n, m, (T)thresh, (const int*)e_col, (const T*)e_cost, (const int*)row_cnt, se, sr, x, y);
@@ -503,6 +545,55 @@ extern "C" int b2t_lap_solve(int dtype, const void* cost, int n, int m, int ld, 
     if (workspace_bytes < b2t_lap_workspace_bytes(dtype, n, m, batch)) return fail(B2T_EINVAL, "b2t_lap_solve: workspace too small");
     if (dtype == B2T_F32) return lap_solve_t<float>((const float*)cost, n, m, ld, thresh, x, y, workspace, batch, s);
     if (dtype == B2T_F64) return lap_solve_t<double>((const double*)cost, n, m, ld, thresh, x, y, workspace, batch, s);
+    return fail(B2T_EINVAL, "dtype must be B2T_F32 or B2T_F64");
+}
+
+extern "C" size_t b2t_lap_csr_workspace_bytes(int batch) { return (size_t)(batch > 0 ? batch : 0) * sizeof(b2t_lap_csr_problem) + 256; }
+
+template <class T>
+static int lap_solve_csr_t(const b2t_lap_csr_problem* probs, int batch, const int* row_start, const int* row_cnt, const int* e_col,
+                           const void* e_cost, const int* e_row, const int* m_col, const void* m_cost, const int* m_row, int* x, int* y,
+                           int* counters, void* ws, cudaStream_t s) {
+    int nmax = 0, mmax = 0, smax = 0, w2max = 0;
+    for (int b = 0; b < batch; ++b) {
+        const b2t_lap_csr_problem& p = probs[b];
+        if (p.n < 0 || p.m < 0 || p.row_off < 0 || p.col_off < 0 || p.entry_off < 0 || p.n_entries < 0 || p.s_cap < 0 ||
+            p.s_cap > p.n_entries || p.w2_base < 0 || p.w2_end < p.w2_base || p.w2_end > p.n_entries)
+            return fail(B2T_EINVAL, "b2t_lap_solve_csr: bad problem descriptor");
+        if (!p.rowwise && (!e_row || (m_col && !m_row)))
+            return fail(B2T_EINVAL, "b2t_lap_solve_csr: an edge-parallel problem (rowwise = 0) needs e_row (and m_row with m_col)");
+        nmax = p.n > nmax ? p.n : nmax; mmax = p.m > mmax ? p.m : mmax; smax = p.s_cap > smax ? p.s_cap : smax;
+        if (p.w2_end - p.w2_base > w2max) w2max = p.w2_end - p.w2_base;
+    }
+    const int w2cap = w2max > 0 ? w2max + 64 : 0;
+    ArenaSize as;
+    LapWork<T>::size(as, nmax, mmax);
+    as.take<int>(smax); as.take<int>(smax); as.take<T>(smax);
+    as.take<int>(w2cap); as.take<int>(w2cap); as.take<T>(w2cap);
+    const size_t smem = as.off + 16;
+    if (smem > 227 * 1024) return fail(B2T_ECAPACITY, "b2t_lap_solve_csr: n, m and the shared-memory windows need more than 227 KB per CTA");
+    b2t_lap_csr_problem* d_probs = (b2t_lap_csr_problem*)align_up((size_t)ws, 256);
+    if (cudaMemcpyAsync(d_probs, probs, sizeof(b2t_lap_csr_problem) * (size_t)batch, cudaMemcpyHostToDevice, s) != cudaSuccess)
+        return fail(B2T_ECUDA, "b2t_lap_solve_csr: cannot upload the problem descriptors");
+    if (!m_col) { m_col = e_col; m_cost = e_cost; m_row = e_row; }
+    auto k = lap_solve_csr_kernel<T>;
+    if (B2T_SET_SMEM(k, smem) != 0) return fail(B2T_ECUDA, "b2t_lap_solve_csr: cannot raise dynamic shared memory");
+    B2T_LAUNCH(k, batch, 512, smem, s, (const b2t_lap_csr_problem*)d_probs, row_start, row_cnt, e_col, (const T*)e_cost, e_row, m_col,
+               (const T*)m_cost, m_row, nmax, mmax, smax, w2cap, x, y, counters);
+    return check_launch("lap_solve_csr");
+}
+
+extern "C" int b2t_lap_solve_csr(int dtype, const b2t_lap_csr_problem* probs_host, int batch, const int* row_start, const int* row_cnt,
+                                 const int* e_col, const void* e_cost, const int* e_row, const int* m_col, const void* m_cost,
+                                 const int* m_row, int* x, int* y, int* counters, void* workspace, size_t workspace_bytes, void* stream) {
+    if (batch < 0 || (batch > 0 && !probs_host)) return fail(B2T_EINVAL, "b2t_lap_solve_csr: bad arguments");
+    if (batch == 0) return B2T_OK;
+    if (workspace_bytes < b2t_lap_csr_workspace_bytes(batch)) return fail(B2T_EINVAL, "b2t_lap_solve_csr: workspace too small");
+    if ((m_col == nullptr) != (m_cost == nullptr))
+        return fail(B2T_EINVAL, "b2t_lap_solve_csr: m_col and m_cost are given together or not at all");
+    cudaStream_t s = (cudaStream_t)stream;
+    if (dtype == B2T_F32) return lap_solve_csr_t<float>(probs_host, batch, row_start, row_cnt, e_col, e_cost, e_row, m_col, m_cost, m_row, x, y, counters, workspace, s);
+    if (dtype == B2T_F64) return lap_solve_csr_t<double>(probs_host, batch, row_start, row_cnt, e_col, e_cost, e_row, m_col, m_cost, m_row, x, y, counters, workspace, s);
     return fail(B2T_EINVAL, "dtype must be B2T_F32 or B2T_F64");
 }
 
