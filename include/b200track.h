@@ -28,7 +28,7 @@ extern "C" {
 
 enum { B2T_F32 = 0, B2T_F64 = 1 };
 enum { B2T_FMT_XYAH = 0, B2T_FMT_XYWH = 1, B2T_FMT_NSA = 2 };
-enum { B2T_SORT = 0, B2T_BYTETRACK = 1, B2T_BOTSORT = 2, B2T_STRONGSORT = 3 };
+enum { B2T_SORT = 0, B2T_BYTETRACK = 1, B2T_BOTSORT = 2, B2T_STRONGSORT = 3, B2T_UAVMOT = 4 };
 enum { B2T_OK = 0, B2T_EINVAL = -1, B2T_ECUDA = -2, B2T_ECAPACITY = -3, B2T_ENOTBUILT = -4 };
 /* 16-bit activation / weight type of the detector branch.  Both feed wgmma at the same rate with fp32
  * accumulation; fp16 (the reference's own GPU half mode, detect.py:41) carries 3 more mantissa bits than bf16. */
@@ -111,7 +111,7 @@ int b2t_lap_solve_csr(int dtype, const b2t_lap_csr_problem* probs_host, int batc
 typedef struct b2t_tracker b2t_tracker;
 
 typedef struct b2t_tracker_config {
-    int kind;          /* B2T_SORT / B2T_BYTETRACK / B2T_BOTSORT / B2T_STRONGSORT */
+    int kind;          /* B2T_SORT / B2T_BYTETRACK / B2T_BOTSORT / B2T_STRONGSORT / B2T_UAVMOT (no features, no camera motion, B2T_F64 only) */
     int dtype;         /* B2T_F32 / B2T_F64 */
     int fmt;           /* Kalman format */
     int n_seq;         /* sequences per launch */
@@ -167,6 +167,13 @@ int b2t_tracker_step_feat(b2t_tracker* t, const float* dets, const int* det_coun
  * b [batch][m][feat_dim] float32, out [batch][n][m] (matching.embedding_distance(metric='euclidean')).  The kernel B2T_STRONGSORT
  * runs before each step; |out - exact| <= gamma_{feat_dim+3} * exact with gamma_k = k u / (1 - k u), u = 2^-53. */
 int b2t_feature_distance(const float* a, int n, const float* b, int m, int feat_dim, double* out, int batch, void* stream);
+/* UAVMOT's structure representation (matching.structure_representation): out[n][3] = [max, min, included angle] over each point's
+ * neighbours at a length in (0, 400), the first index on ties; [1e-4, 1e-4, 1e-4] without neighbours, [max, min, 1e-4] when max ==
+ * min.  dtype B2T_F64: pts [n][2] are track centres (mean[0:2]); B2T_F32: detection centres (get_xy(), float32 lengths).  Device
+ * pointers; the device functions B2T_UAVMOT's step runs. */
+int b2t_structure_vectors(int dtype, const void* pts, int n, double* out, void* stream);
+/* out[n][m] = max(0, cdist(a, b, 'cosine')) for structure vectors a [n][3], b [m][3] (matching.structure_similarity_distance). */
+int b2t_structure_distance(const double* a, int n, const double* b, int m, double* out, void* stream);
 /* Changes theta_iou / theta_emb for the following steps (the reference reads them as plain attributes every frame). */
 int b2t_tracker_set_thetas(b2t_tracker* t, double theta_iou, double theta_emb);
 /* Copies one slot's smoothed feature (feat_dim floats) to the HOST (lazy STrack.features).  Synchronises the stream. */

@@ -24,7 +24,9 @@ class TrackEngine:
         detections' features (step_device(feats=), step_cuda_dets(feats_list=)) and fuses them into associations 1 and 3 with the
         gates theta_iou / theta_emb (set_thetas changes them between steps).
         kind="strongsort" (StrongSORT.update; feat_dim > 0 required, Kalman format 'strongsort' unless given, as track.py:71 forces):
-        the same feature-carrying steps, with the dense cost gamma * IoU distance + (1 - gamma) * Euclidean feature distance."""
+        the same feature-carrying steps, with the dense cost gamma * IoU distance + (1 - gamma) * Euclidean feature distance.
+        kind="uavmot" (UAVMOT.update; float64 only, no features, no camera motion -- use_gmc is not read): ByteTrack's stages with association 1
+        re-solved on 0.98 * IoU distance + 0.02 * structure distance (matching.local_relation_fuse_motion) when its IoU solve matched."""
         if not torch.cuda.is_available():
             raise L.B2TError("TrackEngine needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.lib = L.load()
@@ -328,6 +330,20 @@ class Ops:
         L.check(self.lib, self.lib.b2t_lap_solve(dtype, _dev_ptr(c3), n, m, max(m, 1), float(thresh), _dev_ptr(x), _dev_ptr(y),
                                                  _dev_ptr(workspace), workspace.numel(), bsz, self._s()))
         return (x, y) if batched else (x[0], y[0])
+
+    def structure_vectors(self, pts, detection=False):
+        """pts (n, 2) CUDA tensor -- float64 track centres, or float32 detection centres with detection=True -> (n, 3) float64"""
+        n = pts.shape[0]
+        out = torch.empty((n, 3), dtype=torch.float64, device=self.device)
+        L.check(self.lib, self.lib.b2t_structure_vectors(L.F32 if detection else L.F64, _dev_ptr(pts), n, _dev_ptr(out), self._s()))
+        return out
+
+    def structure_distance(self, a, b):
+        """a (n, 3), b (m, 3) float64 CUDA tensors -> (n, m) float64 max(0, cosine distance)"""
+        n, m = a.shape[0], b.shape[0]
+        out = torch.empty((n, m), dtype=torch.float64, device=self.device)
+        L.check(self.lib, self.lib.b2t_structure_distance(_dev_ptr(a), n, _dev_ptr(b), m, _dev_ptr(out), self._s()))
+        return out
 
 
 _ops = None

@@ -36,7 +36,8 @@ class TrackingPipeline:
         Frames must then be uint8 (the crops come from det.src_u8).
         StrongSORT (engine kind "strongsort", feat_dim 512): reid must be a ``b200track.osnet.OsnetExtractor`` and gmc an
         ``EccEstimator`` for the source-frame size, or None for use_ECC=False; reid_cap defaults to min(n_seq * dmax, 1024).  A
-        StrongSORT engine with a ReidExtractor or a GmcEstimator, and an OsnetExtractor or EccEstimator with another engine, raise."""
+        StrongSORT engine with a ReidExtractor or a GmcEstimator, and an OsnetExtractor or EccEstimator with another engine, raise.
+        UAVMOT (engine kind "uavmot") takes neither reid nor gmc."""
         self.dets = list(detector) if isinstance(detector, (list, tuple)) else [detector]
         if len(self.dets) not in (1, 2):
             raise L.B2TError("TrackingPipeline takes one detector or two twins")
@@ -59,6 +60,8 @@ class TrackingPipeline:
         if gmc is not None and ss != isinstance(gmc, EccEstimator):
             raise L.B2TError("TrackingPipeline: %s takes %s for gmc= (got %s)" % ("StrongSORT" if ss else engine.kind,
                              "an EccEstimator" if ss else "a GmcEstimator", type(gmc).__name__))
+        if engine.kind == "uavmot" and gmc is not None:        # UAVMOT.update has no camera-motion step
+            raise L.B2TError("TrackingPipeline: a UAVMOT engine takes no gmc= (got %s)" % type(gmc).__name__)
         self.ecc, self.ss = (gmc if ss else None), ss
         dev = det.dev
         self.dev = dev

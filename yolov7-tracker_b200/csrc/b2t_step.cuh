@@ -4,6 +4,8 @@
 //   BaseTracker.update   tracker/basetrack.py:368-487   (kind 0, SORT)
 //   ByteTrack.update     tracker/bytetrack.py:41-204    (kind 1)
 //   BoTSORT.update       tracker/botsort.py:313-493     (kind 2, + multi_gmc :250-269)
+//   StrongSORT.update    tracker/strongsort.py:91-250   (kind 3, track_step_ss_kernel)
+//   UAVMOT.update        tracker/uavmot.py:106-279      (kind 4, track_step_uav_kernel)
 // including STrack.activate / update / re_activate / multi_predict (basetrack.py:222-339) and
 // joint_stracks / sub_stracks / remove_duplicate_stracks (:540-576).  oracle/trackers.py is the
 // CPU statement of the same machine; the quirk numbers (q3..q13) refer to SURVEY.md section 8a.
@@ -26,7 +28,7 @@
 
 namespace b2t {
 
-enum { KIND_SORT = 0, KIND_BYTETRACK = 1, KIND_BOTSORT = 2 };
+enum { KIND_SORT = 0, KIND_BYTETRACK = 1, KIND_BOTSORT = 2, KIND_STRONGSORT = 3, KIND_UAVMOT = 4 };
 enum { ST_NEW = 0, ST_TRACKED = 1, ST_LOST = 2, ST_REMOVED = 3 };
 enum { CTRL_FRAME = 0, CTRL_NEXT_ID = 1, CTRL_NTRACKED = 2, CTRL_NLOST = 3, CTRL_NFREE = 4, CTRL_ERR = 5 };
 enum { STAT_NOUT = 0, STAT_NEXT_ID = 1, STAT_NTRACKED = 2, STAT_NLOST = 3, STAT_ERR = 4, STAT_FRAME = 5,
@@ -174,6 +176,87 @@ struct AppCtx {
     const int* col_det;     // [m] detection row of each column (its feature is feats[det])
     const float* feats;     // this sequence's [dmax][feat_dim] detection features
     double theta_iou, theta_emb;
+    static constexpr bool kStruct = false;
+};
+
+// UAVMOT's structure cost (matching.py:284-386, SURVEY q22).  Each point of a set (the pool's predicted centres mean[0:2] in
+// float64, the high detections' get_xy() = tl + wh // 2 in float32) is described by [max, min, angle] over the other points B at a
+// length 0 < |AB| < 400: the longest and the shortest such length (first index on ties) and the included angle between the offsets to
+// those two points; [1e-4, 1e-4, 1e-4] without neighbours, [max, min, 1e-4] when max == min.  S(i, j) = max(0, cosine distance).
+constexpr double UAV_LOCAL_R = 400.0, UAV_LAMBDA = 0.98, UAV_T1 = 0.8;
+
+// np.linalg.norm([|dx|, |dy|]) as the host evaluates it: float64 goes through BLAS ddot, whose two-element tail is dx * dx followed
+// by one fused multiply-add; float32 through sdot in separate float32 operations.  Compared as rounded lengths, never as squares:
+// two different sums can round to the same length, and the reference then takes the first index.
+B2T_DEV double uav_len(double dx, double dy) { return sqrt(fma(dy, dy, dx * dx)); }
+B2T_DEV float uav_len(float dx, float dy) { return sqrtf(dx * dx + dy * dy); }
+
+// int(math.atan2(dy, dx) * 180 / math.pi) (matching.py:330-335) for an offset that is not (0, 0).  On the axes and diagonals the
+// host's value is an exact integer (0, +-45, +-90, +-135, 180) and is returned as such: CUDA's atan2 (2 ulp) may fall one ulp below
+// it, and int() truncates.  Elsewhere the host value stays further from an integer than that error (tests/test_uavmot_angles.py).
+B2T_DEV int uav_direction(double dx, double dy) {
+    if (dy == 0.0) return dx > 0.0 ? 0 : 180;           // dy is +0 here (a difference of equal values), so atan2 gives +pi
+    if (dx == 0.0) return dy > 0.0 ? 90 : -90;
+    if (fabs(dx) == fabs(dy)) return dx > 0.0 ? (dy > 0.0 ? 45 : -45) : (dy > 0.0 ? 135 : -135);
+    return (int)(atan2(dy, dx) * 180.0 / 3.141592653589793);
+}
+
+B2T_DEV int uav_included_angle(int a1, int a2) {
+    if (a1 * a2 >= 0) return a1 > a2 ? a1 - a2 : a2 - a1;
+    const int inc = (a1 < 0 ? -a1 : a1) + (a2 < 0 ? -a2 : a2);
+    return inc > 180 ? 360 - inc : inc;
+}
+
+// structure_representation over pts[0..n) (x, y pairs of P = double for tracks, float for detections) -> sv[n][3], one warp per point.
+template <class P> B2T_DEV void uav_structure(const P* pts, int n, double* sv) {
+    const int lane = lane_id();
+    for (int i = warp_id(); i < n; i += num_warps()) {
+        const P ax = pts[2 * i], ay = pts[2 * i + 1];
+        P lmax = (P)0, lmin = (P)0;
+        int imax = -1, imin = -1;
+        for (int j = lane; j < n; j += 32) {           // per lane in ascending j: strict compares keep the first index
+            const P l = uav_len(ax - pts[2 * j], ay - pts[2 * j + 1]);
+            if (l < (P)UAV_LOCAL_R && l > (P)0) {
+                if (imax < 0 || l > lmax) { lmax = l; imax = j; }
+                if (imin < 0 || l < lmin) { lmin = l; imin = j; }
+            }
+        }
+        for (int o = 16; o; o >>= 1) {
+            const P ol = shfl_xor(lmax, o), on = shfl_xor(lmin, o);
+            const int oi = shfl_xor(imax, o), oj = shfl_xor(imin, o);
+            if (oi >= 0 && (imax < 0 || ol > lmax || (ol == lmax && oi < imax))) { lmax = ol; imax = oi; }
+            if (oj >= 0 && (imin < 0 || on < lmin || (on == lmin && oj < imin))) { lmin = on; imin = oj; }
+        }
+        if (lane == 0) {
+            double* o = sv + 3 * i;
+            if (imax < 0) { o[0] = 1e-4; o[1] = 1e-4; o[2] = 1e-4; }
+            else if (lmax == lmin) { o[0] = (double)lmax; o[1] = (double)lmin; o[2] = 1e-4; }
+            else {
+                const int a1 = uav_direction((double)(pts[2 * imax] - ax), (double)(pts[2 * imax + 1] - ay));
+                const int a2 = uav_direction((double)(pts[2 * imin] - ax), (double)(pts[2 * imin + 1] - ay));
+                o[0] = (double)lmax; o[1] = (double)lmin; o[2] = (double)uav_included_angle(a1, a2);
+            }
+        }
+    }
+}
+
+// max(0, cdist(u, v, 'cosine')) in SciPy's order: row norms sqrt(u0 u0 + u1 u1 + u2 u2), then 1 - clip(u.v / (|u| |v|), -1, 1)
+B2T_DEV double uav_struct_dist(const double* u, const double* v) {
+    const double nu = sqrt(u[0] * u[0] + u[1] * u[1] + u[2] * u[2]);
+    const double nv = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+    double c = (u[0] * v[0] + u[1] * v[1] + u[2] * v[2]) / (nu * nv);
+    if (fabs(c) > 1.0) c = copysign(1.0, c);
+    const double d = 1.0 - c;
+    return d > 0.0 ? d : 0.0;
+}
+
+// The cost hook of UAVMOT's second association-1 solve: lambda * IoU distance + (1 - lambda) * S (local_relation_fuse_motion,
+// matching.py:308; 1 - 0.98 = 0.020000000000000018).  S >= 0, so a pair that does not overlap costs >= 0.98 > 0.8: the candidates
+// are still the overlapping pairs build_csr finds.
+struct StructCtx {
+    const double* sv_row;   // [n][3] structure vectors of the rows (the pool)
+    const double* sv_col;   // [m][3] ... of the columns (the high detections)
+    static constexpr bool kStruct = true;
 };
 
 // Stage 2b of build_csr: one warp per listed edge (list[q] = edge index, top bit set when the edge lives in the global workspace
@@ -213,15 +296,19 @@ B2T_DEVNI int app_costs(const AppCtx app, const float* tfeat, int D, const int* 
     return lowered;
 }
 
-template <class T>
+template <class X> struct NoDeduce { using type = X; };
+
+// Ctx = StructCtx: UAVMOT's fused cost replaces the IoU distance of every candidate (app is then that context, never null).
+template <class T, class Ctx = AppCtx>
 B2T_DEVNI bool build_csr(SeqView<T>& v, StepSmem<T>& sm, int n, int m, T thresh, int* dbg = nullptr, long long* dbgt = nullptr,
-                         const AppCtx* app = nullptr) {
+                         const typename NoDeduce<Ctx>::type* app = nullptr) {
+    constexpr bool STRUCT = Ctx::kStruct;
     const int tid = (int)threadIdx.x, nthr = (int)blockDim.x, lane = lane_id();
     int* misc = sm.misc;
     const T* colbox = sm.colbox;
     const bool sorted = m > 64;
     T xmin = (T)0, scale = (T)0, maxw = (T)0;
-    if (tid == 0) { misc[50] = 0; misc[51] = 0; if (app) misc[53] = 0; }
+    if (tid == 0) { misc[50] = 0; misc[51] = 0; if (!STRUCT && app) misc[53] = 0; }
     if (sorted) {
         // ---- column statistics: min / max x1, max width
         T lo = (T)1e30, hi = (T)-1e30, mw = (T)0;
@@ -341,6 +428,20 @@ B2T_DEVNI bool build_csr(SeqView<T>& v, StepSmem<T>& sm, int n, int m, T thresh,
         }
         return i;
     };
+    if constexpr (STRUCT) {
+        for (int e = tid; e < nE; e += nthr) {
+            int* pc; T* pw;
+            const int i = locate(e, pc, pw);
+            const int j = pc[e];
+            const T iou_d = (T)1 - iou_plus1<T>(sm.rowbox + 4 * i, colbox + 4 * j);
+            const T cost = (T)(UAV_LAMBDA * (double)iou_d + (1.0 - UAV_LAMBDA) * uav_struct_dist(app->sv_row + 3 * i, app->sv_col + 3 * j));
+            if (cost < thresh) pw[e] = cost;
+            else pc[e] = -1;
+        }
+        __syncthreads();
+        B2T_SUB(5);
+        return fits;
+    } else {
     const T th_iou = app ? (T)app->theta_iou : (T)0;
     for (int e = tid; e < nE; e += nthr) {
         int* pc; T* pw;
@@ -362,6 +463,7 @@ B2T_DEVNI bool build_csr(SeqView<T>& v, StepSmem<T>& sm, int n, int m, T thresh,
     }
     B2T_SUB(5);
     return fits;
+    }
 }
 
 // StrongSORT's fused cost (strongsort.py:150-157, :206-208): gamma * IoU distance + (1 - gamma) * App, with App the Euclidean distance
@@ -423,6 +525,10 @@ B2T_DEVNI bool build_csr_dense(SeqView<T>& v, StepSmem<T>& sm, int n, int m, T t
     return fits;
 }
 
+// UAVMOT's per-sequence scratch in the state block, in doubles: pool centres [cap][2] double, high-detection centres [dmax][2] float,
+// structure vectors [cap][3] and [dmax][3] double.  Only the UAVMOT kind has it; the other kinds' shared memory is unchanged.
+__host__ __device__ inline size_t uav_seq_doubles(int cap, int dmax) { return (size_t)5 * cap + (size_t)4 * dmax; }
+
 template <class T> struct StepCtx {
     SeqView<T> v;
     StepSmem<T> sm;
@@ -448,14 +554,15 @@ template <class T> B2T_DEV LapCsr<T> step_csr(StepCtx<T>& c, int w2_base = 0, in
 }
 
 // DENSE: the candidates are every pair whose StrongSORT cost is below thresh (build_csr_dense, *dense), not the overlapping ones.
-template <class T, bool DENSE = false> B2T_DEVNI void associate(StepCtx<T>& c, int n, int m, T thresh, int* err, long long* tsplit,
-                                                                int* dbg = nullptr, const AppCtx* app = nullptr,
-                                                                const DenseCtx* dense = nullptr) {
+// Ctx = StructCtx: UAVMOT's fused cost over the overlapping pairs (build_csr's cost hook, *app).
+template <class T, bool DENSE = false, class Ctx = AppCtx>
+B2T_DEVNI void associate(StepCtx<T>& c, int n, int m, T thresh, int* err, long long* tsplit, int* dbg = nullptr,
+                         const typename NoDeduce<Ctx>::type* app = nullptr, const DenseCtx* dense = nullptr) {
     StepSmem<T>& sm = c.sm;
     long long dt = phase_clock();
     bool ok;
     if constexpr (DENSE) ok = build_csr_dense<T>(c.v, sm, n, m, thresh, *dense);
-    else ok = build_csr<T>(c.v, sm, n, m, thresh, dbg, &dt, app);
+    else ok = build_csr<T, Ctx>(c.v, sm, n, m, thresh, dbg, &dt, app);
     if (!ok && threadIdx.x == 0) *err |= ERR_EDGES;
     // The rows that did not fit the shared-memory edge mirror live in the global edge workspace.  rowbox / colbox are dead from
     // here to the next association (each one refills them): the first spilled rows are copied into that memory, so that the
@@ -586,11 +693,14 @@ B2T_DEVNI void copy_features(float* tfeat, int D, const int* slots, const int* d
 // same code as without appearance support.
 // SS (with APP): StrongSORT.update (strongsort.py:91-250).  dist_all [S][cap][dmax] holds the Euclidean distances feat_dist_kernel
 // computed for this frame (tracked and lost lists at frame start x detection rows); gamma weighs the IoU distance in the fused cost.
-template <class T, bool APP, bool SS = false>
+// UAV (without APP): UAVMOT.update (uavmot.py:106-279).  uav_all [S][uav_seq_doubles(cap, dmax)] is the per-sequence scratch of the
+// structure vectors (uav_seq_doubles); the association-2 stage and the list algebra are StrongSORT's (q21 is q18).
+template <class T, bool APP, bool SS = false, bool UAV = false>
 B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq, const float* dets_all,
                             const int* det_count, const float* feats_all, const double* warps, const int* id_base, double* out_all,
                             int out_rows, int* stat_all, unsigned char* smem_raw, const double* dist_all = nullptr,
-                            double gamma = 0.0) {
+                            double gamma = 0.0, double* uav_all = nullptr) {
+    constexpr bool Q18 = SS || UAV;     // u_tracks1_idx indexes u_tracks0 but marks strack_pool[idx] lost (strongsort.py:195, uavmot.py:228)
     StepCtx<T> c(st, seq, prm);
     Arena arena(smem_raw);
     c.sm.carve(arena, st.cap, st.dmax, st.esm);
@@ -728,7 +838,41 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
             const DenseCtx d1 = {sm.pool, sm.hi, dist, st.dmax, gamma};
             associate<T, true>(c, npool, nhi, (T)p.t1, err, &tsplit, stat + STAT_SUB0, nullptr, &d1);
         } else {
+            if constexpr (UAV) for (int k = tid; k < npool; k += nthr) sm.dupa[k] = 0;
             associate<T>(c, npool, nhi, (T)p.t1, err, &tsplit, stat + STAT_SUB0, feats ? &app1 : nullptr);
+        }
+        if constexpr (UAV) {
+            // q20 (uavmot.py:184): the IoU solve at 0.7 only decides whether the fused solve runs -- it does when matched_pair0.any(),
+            // i.e. some match other than the single pair (0, 0); the fused solve at 0.8 then replaces its result
+            const int* x0 = sm.lap.x;
+            const int any = block_compact(npool, [&](int i) { return x0[i] >= 0 && (i != 0 || x0[i] != 0); }, sm.ntr, sm.misc);
+            if (any > 0) {
+                double* ws = uav_all + (size_t)seq * uav_seq_doubles(cap, st.dmax);
+                double* tp = ws;                                              // [cap][2] pool centres
+                float* dp = reinterpret_cast<float*>(ws + 2 * cap);           // [dmax][2] high-detection centres
+                double* sv_t = ws + 2 * cap + st.dmax;                         // [cap][3]
+                double* sv_d = sv_t + 3 * cap;                                 // [dmax][3]
+                for (int k = tid; k < npool; k += nthr) {
+                    const T* mu = v.mean + (size_t)sm.pool[k] * 8;
+                    tp[2 * k] = (double)mu[0]; tp[2 * k + 1] = (double)mu[1];
+                }
+                for (int k = tid; k < nhi; k += nthr) {        // AMF_STrack.get_xy: tlwh2xywh(tlwh)[:2] = tl + wh // 2, float32 (q2)
+                    const float* d = dets + 6 * sm.hi[k];
+                    dp[2 * k] = d[0] + floorf((d[2] - d[0]) * 0.5f);
+                    dp[2 * k + 1] = d[1] + floorf((d[3] - d[1]) * 0.5f);
+                }
+                __syncthreads();
+                uav_structure<double>(tp, npool, sv_t);
+                uav_structure<float>(dp, nhi, sv_d);
+                // the solve left rowbox / colbox to its edge window: refill them
+                fill_track_boxes<T>(v, p.fmt, sm.pool, npool, sm.rowbox);
+                for (int k = tid; k < nhi; k += nthr)
+                    for (int q = 0; q < 4; ++q) sm.colbox[4 * k + q] = sm.detbox[4 * sm.hi[k] + q];
+                __syncthreads();
+                const StructCtx sc = {sv_t, sv_d};
+                // its CSR / LAP boundary ends phase 4 and its LAP is phase 5: the two solves and the structure scans are all counted
+                associate<T, false, StructCtx>(c, npool, nhi, (T)UAV_T1, err, &tsplit, stat + STAT_SUB0, &sc);
+            }
         }
         if (tid == 0) { stat[STAT_PHASE0 + 4] = (int)(tsplit - tprev); tprev = tsplit;
                         stat[12] = sm.lap.scratch[45]; stat[13] = sm.lap.scratch[41]; stat[14] = sm.lap.scratch[43]; stat[15] = sm.misc[50]; }
@@ -745,7 +889,7 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         int nut;
         if (sort)
             nut = block_compact(npool, [&](int i) { return x[i] < 0 && sm.pstate[i] == ST_TRACKED; }, sm.ut, sm.misc);
-        else if (SS || p.kind == KIND_BYTETRACK)     // strongsort.py:183: only the Tracked leftovers go on
+        else if (Q18 || p.kind == KIND_BYTETRACK)    // strongsort.py:171, uavmot.py:205: only the Tracked leftovers go on
             nut = block_compact(npool, [&](int i) { return x[i] < 0 && sm.pstate[i] == ST_TRACKED; }, sm.ut, sm.misc);
         else
             nut = block_compact(npool, [&](int i) { return x[i] < 0; }, sm.ut, sm.misc);
@@ -759,28 +903,29 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         apply_matches<T>(c, sm.pool, npool, dets, sm.ntr, sm.used);
         if (feats) ema_features(v.feat, v.feat_dim, sm.pool, npool, feats, sm.ntr, sm.used);
         B2T_PHASE(6);
-        if constexpr (SS) {
+        if constexpr (Q18) {
             for (int k = tid; k < npool; k += nthr)
                 if (x[k] >= 0) sm.dupa[k] = sm.pstate[k] == ST_TRACKED ? 1 : 2;
-            // ---- association 2 (strongsort.py:180-198): u_tracks0 (Tracked leftovers) x the leftover detections, IoU only, 0.5
+            // ---- association 2, IoU only, 0.5: u_tracks0 (Tracked leftovers) x the leftover high detections (strongsort.py:174-191)
+            // or x the low detections (uavmot.py:211-224)
             for (int k = tid; k < nut; k += nthr) sm.nlo[k] = sm.pool[sm.ut[k]];
             __syncthreads();
             fill_track_boxes<T>(v, p.fmt, sm.nlo, nut, sm.rowbox);
-            for (int k = tid; k < nud0; k += nthr)
-                for (int q = 0; q < 4; ++q) sm.colbox[4 * k + q] = sm.detbox[4 * sm.udets0[k] + q];
+            for (int k = tid; k < (SS ? nud0 : nlo); k += nthr)
+                for (int q = 0; q < 4; ++q) sm.colbox[4 * k + q] = sm.detbox[4 * (SS ? sm.udets0 : sm.lo)[k] + q];
             __syncthreads();
-            associate<T>(c, nut, nud0, (T)p.t2, err, nullptr);
+            associate<T>(c, nut, SS ? nud0 : nlo, (T)p.t2, err, nullptr);
             for (int k = tid; k < nut; k += nthr) {
                 const int xx = x[k];
-                sm.ntr[k] = xx >= 0 ? sm.udets0[xx] : -1;
+                sm.ntr[k] = xx >= 0 ? (SS ? sm.udets0 : sm.lo)[xx] : -1;
                 sm.used[k] = 0;
                 if (xx >= 0) sm.dupa[sm.ut[k]] |= 4;
             }
             __syncthreads();
             apply_matches<T>(c, sm.nlo, nut, dets, sm.ntr, sm.used);
-            ema_features(v.feat, v.feat_dim, sm.nlo, nut, feats, sm.ntr, sm.used);    // every StrongSORT detection has a feature
-            // q18 (strongsort.py:195-198): u_tracks1_idx indexes u_tracks0, but the track marked lost is strack_pool[idx] -- possibly
-            // one updated or re-activated this frame.  The track that really went unmatched stays Tracked.
+            if constexpr (SS) ema_features(v.feat, v.feat_dim, sm.nlo, nut, feats, sm.ntr, sm.used);    // every StrongSORT detection has a feature
+            // q18 / q21 (strongsort.py:195-198, uavmot.py:228-231): u_tracks1_idx indexes u_tracks0, but the track marked lost is
+            // strack_pool[idx] -- possibly one updated or re-activated this frame.  The track that really went unmatched stays Tracked.
             for (int k = tid; k < nut; k += nthr)
                 if (x[k] < 0) { v.state[sm.pool[k]] = ST_LOST; sm.dupa[k] |= 8; }
             __syncthreads();
@@ -789,12 +934,14 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
             nlostnow = block_compact(nut, [&](int k) { return x[k] < 0 && !(sm.pstate[k] == ST_LOST && sm.dupa[k] == 8); },
                                      sm.ut, sm.misc);
             for (int k = tid; k < nlostnow; k += nthr) sm.lost_now[k] = sm.pool[sm.ut[k]];
-            // u_det1: the detections association 2 left, for association 3
-            const int nud1 = block_compact(nud0, [&](int j) { return y[j] < 0; }, sm.lo, sm.misc);
-            for (int k = tid; k < nud1; k += nthr) sm.hi[k] = sm.udets0[sm.lo[k]];
-            __syncthreads();
-            for (int k = tid; k < nud1; k += nthr) sm.udets0[k] = sm.hi[k];
-            nud0 = nud1;
+            if constexpr (SS) {
+                // u_det1: the detections association 2 left, for association 3 (UAVMOT's association 3 takes association 1's)
+                const int nud1 = block_compact(nud0, [&](int j) { return y[j] < 0; }, sm.lo, sm.misc);
+                for (int k = tid; k < nud1; k += nthr) sm.hi[k] = sm.udets0[sm.lo[k]];
+                __syncthreads();
+                for (int k = tid; k < nud1; k += nthr) sm.udets0[k] = sm.hi[k];
+                nud0 = nud1;
+            }
             __syncthreads();
         } else if (sort) {
             // basetrack.py:429-433: unmatched Tracked rows become lost
@@ -907,8 +1054,8 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
     // ---- P9: list algebra (bytetrack.py:186-193)
     int nt1 = block_compact(n_tracked0, [&](int k) { return v.state[v.tracked[k]] == ST_TRACKED; }, sm.ut, sm.misc);
     for (int k = tid; k < nt1; k += nthr) sm.ntr[k] = v.tracked[sm.ut[k]];
-    if constexpr (SS) {
-        // joint_stracks(tracked, activated_starcks) (strongsort.py:233): an updated track that q18 marked lost left the filtered
+    if constexpr (Q18) {
+        // joint_stracks(tracked, activated_starcks) (strongsort.py:233, uavmot.py:262): an updated track that q18 marked lost left the filtered
         // list and comes back here, in activated_starcks order -- association 1's updates, then association 2's
         if (!p.predict_only) {
             for (int bit = 1; bit <= 4; bit += 3) {
@@ -923,9 +1070,9 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
     nt1 += nbirth + nref;
     if (nt1 > cap) { nt1 = cap; if (tid == 0) *err |= ERR_SLOTS; }
     // old lost entries that were not re-found and whose id was not in the removed list before this frame
-    // (StrongSORT: "not re-found" is frame_id != f -- a re-found track that q18 marked lost is Lost again, yet on the tracked list)
+    // (StrongSORT, UAVMOT: "not re-found" is frame_id != f -- a re-found track that q18 marked lost is Lost again, yet on the tracked list)
     int nl1 = block_compact(n_lost0, [&](int k) { const int s = v.lost[k];
-        return (SS ? v.frame_id[s] != f : v.state[s] != ST_TRACKED) && !(v.removed_at[s] != 0 && v.removed_at[s] < f); }, sm.ut, sm.misc);
+        return (Q18 ? v.frame_id[s] != f : v.state[s] != ST_TRACKED) && !(v.removed_at[s] != 0 && v.removed_at[s] < f); }, sm.ut, sm.misc);
     for (int k = tid; k < nl1; k += nthr) sm.nlo[k] = v.lost[sm.ut[k]];
     __syncthreads();
     const int nl_add = block_compact(nlostnow, [&](int k) { const int s = sm.lost_now[k];

@@ -370,6 +370,28 @@ track_step_ss_kernel(TrackState st, StepParams prm, const float* dets, const int
                                   dist, gamma);
 }
 
+// UAVMOT (B2T_UAVMOT): its own kernel too, float64 only (check_cfg).  uav [S][uav_seq_doubles(cap, dmax)] is the structure-vector
+// scratch.
+template <class T>
+__global__ void __launch_bounds__(512, 1)
+track_step_uav_kernel(TrackState st, StepParams prm, const float* dets, const int* det_count, const int* id_base, double* out,
+                      int out_rows, int* stat, double* uav) {
+    B2T_DYN_SMEM(smem_raw);
+    track_step_cta<T, false, false, true>(st, prm, (int)blockIdx.x, dets, det_count, nullptr, nullptr, id_base, out, out_rows, stat,
+                                          smem_raw, nullptr, 0.0, uav);
+}
+
+// b2t_structure_vectors / b2t_structure_distance: the step's own device functions on caller-given sets, one CTA / one thread per pair
+template <class P>
+__global__ void __launch_bounds__(512) structure_vectors_kernel(const P* pts, int n, double* out) { uav_structure<P>(pts, n, out); }
+
+__global__ void structure_distance_kernel(const double* a, int n, const double* b, int m, double* out) {
+    const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= (long long)n * m) return;
+    const int i = (int)(q / m), j = (int)(q % m);
+    out[q] = uav_struct_dist(a + 3 * (size_t)i, b + 3 * (size_t)j);
+}
+
 __global__ void track_reset_kernel(TrackState st) {
     const int s = (int)blockIdx.x;
     const size_t o = (size_t)s * st.cap;
@@ -606,6 +628,7 @@ struct b2t_tracker {
     // device staging for the *_host entry point (inside the state block)
     float* d_dets; int* d_count; double* d_warps; int* d_idbase; double* d_out; int* d_stat; double* d_slot; double* d_list;
     double* dist;   // B2T_STRONGSORT: [S][cap][dmax] feature distances of the current frame
+    double* uav;    // B2T_UAVMOT: [S][uav_seq_doubles(cap, dmax)] structure-vector scratch
     size_t out_rows_cap;
 };
 
@@ -639,16 +662,21 @@ static void layout(const b2t_tracker_config& c, unsigned char* base, b2t_tracker
         TAKE(st.e_app, int, S * (size_t)c.ecap);
     }
     if (c.kind == B2T_STRONGSORT) { TAKE(dist, double, S * cap * (size_t)c.dmax); }
+    if (c.kind == B2T_UAVMOT) { TAKE(uav, double, S * uav_seq_doubles(c.cap, c.dmax)); }
 #undef TAKE
     *total = align_up(L.off, 256);
 }
 
 static int check_cfg(const b2t_tracker_config* c) {
     if (!c) return fail(B2T_EINVAL, "null config");
-    if (c->kind < 0 || c->kind > 3 || c->fmt < 0 || c->fmt > 2 || (c->dtype != B2T_F32 && c->dtype != B2T_F64))
+    if (c->kind < 0 || c->kind > 4 || c->fmt < 0 || c->fmt > 2 || (c->dtype != B2T_F32 && c->dtype != B2T_F64))
         return fail(B2T_EINVAL, "b2t_tracker: bad kind / fmt / dtype");
     if (c->n_seq < 1 || c->cap < 64 || c->dmax < 1 || c->dmax > 1024 || c->cap > 4096 || c->ecap < 1)
         return fail(B2T_EINVAL, "b2t_tracker: bad n_seq / cap (64..4096) / dmax (1..1024) / ecap");
+    // the float32 build of the fused step has a derived rounding bound (tests/step_bounds.py) that does not cover UAVMOT's structure
+    // cost and its second solve yet: the kind runs in float64 only
+    if (c->kind == B2T_UAVMOT && c->dtype != B2T_F64)
+        return fail(B2T_EINVAL, "b2t_tracker: B2T_UAVMOT is built for dtype B2T_F64 only");
     if (c->kind == B2T_STRONGSORT) {
         if (c->feat_dim <= 0) return fail(B2T_EINVAL, "b2t_tracker: B2T_STRONGSORT needs appearance features (feat_dim > 0)");
         if (!(c->gamma >= 0.0 && c->gamma <= 1.0)) return fail(B2T_EINVAL, "b2t_tracker: gamma must lie in [0, 1]");
@@ -703,16 +731,19 @@ extern "C" int b2t_tracker_create(const b2t_tracker_config* cfg, void* state_mem
     p.new_thresh = (float)(cfg->conf_thresh + 0.1);                                           // bytetrack.py:175
     if (cfg->kind == B2T_SORT) { p.t1 = cfg->iou_thresh; p.t2 = 0.0; p.t3 = cfg->iou_thresh + 0.1; }   // basetrack.py:414,438
     else if (cfg->kind == B2T_STRONGSORT) { p.t1 = 0.7; p.t2 = 0.5; p.t3 = 0.7; }           // strongsort.py:158,185,209
+    else if (cfg->kind == B2T_UAVMOT) { p.t1 = 0.7; p.t2 = 0.5; p.t3 = 0.7; }               // uavmot.py:182,212,235 (the fused solve: 0.8)
     else { p.t1 = 0.9; p.t2 = 0.5; p.t3 = 0.7; }                                              // bytetrack.py:118,137,160
     p.t_dup = 0.15;                                                                           // basetrack.py:565
     p.max_time_lost = (int)(cfg->frame_rate / 30.0 * cfg->track_buffer);                      // basetrack.py:355-356
-    p.use_gmc = cfg->use_gmc; p.predict_only = 0;
+    p.use_gmc = cfg->kind == B2T_UAVMOT ? 0 : cfg->use_gmc; p.predict_only = 0;             // UAVMOT has no camera-motion step
     p.theta_iou = cfg->theta_iou; p.theta_emb = cfg->theta_emb;                               // botsort.py:289
     t->smem = cfg->dtype == B2T_F64 ? StepSmem<double>::bytes(cfg->cap, cfg->dmax, t->st.esm) : StepSmem<float>::bytes(cfg->cap, cfg->dmax, t->st.esm);
     const bool app = cfg->feat_dim > 0;
     int rs;
     if (cfg->kind == B2T_STRONGSORT)
         rs = cfg->dtype == B2T_F64 ? B2T_SET_SMEM((track_step_ss_kernel<double>), t->smem) : B2T_SET_SMEM((track_step_ss_kernel<float>), t->smem);
+    else if (cfg->kind == B2T_UAVMOT)
+        rs = B2T_SET_SMEM((track_step_uav_kernel<double>), t->smem);
     else if (cfg->dtype == B2T_F64) rs = app ? B2T_SET_SMEM((track_step_kernel<double, true>), t->smem) : B2T_SET_SMEM((track_step_kernel<double, false>), t->smem);
     else rs = app ? B2T_SET_SMEM((track_step_kernel<float, true>), t->smem) : B2T_SET_SMEM((track_step_kernel<float, false>), t->smem);
     if (rs != 0) { delete t; return fail(B2T_ECUDA, "cannot raise dynamic shared memory"); }
@@ -747,6 +778,9 @@ static int step_launch(b2t_tracker* t, const float* dets, const int* det_count, 
             auto k = track_step_ss_kernel<float>;
             B2T_LAUNCH(k, c.n_seq, 512, t->smem, s, t->st, p, dets, det_count, feats, warps, id_base, out, out_rows, stat, t->dist, c.gamma);
         }
+    } else if (t->cfg.kind == B2T_UAVMOT) {
+        auto k = track_step_uav_kernel<double>;
+        B2T_LAUNCH(k, t->cfg.n_seq, 512, t->smem, s, t->st, p, dets, det_count, id_base, out, out_rows, stat, t->uav);
     } else if (t->cfg.dtype == B2T_F64) {
         auto k = app ? track_step_kernel<double, true> : track_step_kernel<double, false>;
         B2T_LAUNCH(k, t->cfg.n_seq, 512, t->smem, s, t->st, p, dets, det_count, feats, warps, id_base, out, out_rows, stat);
@@ -771,6 +805,25 @@ extern "C" int b2t_tracker_step_feat(b2t_tracker* t, const float* dets, const in
     if (!predict_only && !feats) return fail(B2T_EINVAL, "b2t_tracker_step_feat: feats is NULL");
     if (((size_t)feats & 15) != 0) return fail(B2T_EINVAL, "b2t_tracker_step_feat: feats must be 16-B aligned");
     return step_launch(t, dets, det_count, feats, warps, id_base, out, out_rows, stat, predict_only, stream);
+}
+
+extern "C" int b2t_structure_vectors(int dtype, const void* pts, int n, double* out, void* stream) {
+    if (n < 0 || (n > 0 && (!pts || !out))) return fail(B2T_EINVAL, "b2t_structure_vectors: bad arguments");
+    if (n == 0) return B2T_OK;
+    cudaStream_t s = (cudaStream_t)stream;
+    DISPATCH(dtype,
+        B2T_LAUNCH(structure_vectors_kernel<float>, 1, 512, 0, s, (const float*)pts, n, out),
+        B2T_LAUNCH(structure_vectors_kernel<double>, 1, 512, 0, s, (const double*)pts, n, out));
+    return check_launch("structure_vectors");
+}
+
+extern "C" int b2t_structure_distance(const double* a, int n, const double* b, int m, double* out, void* stream) {
+    if (n < 0 || m < 0 || (n > 0 && m > 0 && (!a || !b || !out))) return fail(B2T_EINVAL, "b2t_structure_distance: bad arguments");
+    if (n == 0 || m == 0) return B2T_OK;
+    const long long q = (long long)n * m;
+    if ((q + 255) / 256 > 2147483647LL) return fail(B2T_EINVAL, "b2t_structure_distance: n * m too large for one launch");
+    B2T_LAUNCH(structure_distance_kernel, (int)((q + 255) / 256), 256, 0, (cudaStream_t)stream, a, n, b, m, out);
+    return check_launch("structure_distance");
 }
 
 extern "C" int b2t_tracker_set_thetas(b2t_tracker* t, double theta_iou, double theta_emb) {

@@ -6,8 +6,10 @@ GPU-backed (libb200track.so):
   buffered_iou_distance        reference :391-407 -> b2t_iou_cost
   fuse_motion                  reference :202-213 -> b2t_kalman_gating
   matching_cascade             reference :216-279 -> linear_assignment per level
-Appearance costs (cosine / euclidean GEMMs, out of the section-8 hot path) run on the GPU through torch;
-the UAVMOT structure costs are not provided (NotImplementedError).
+  structure_representation     reference :344-386 -> b2t_structure_vectors   (UAVMOT; the step's own device functions)
+  structure_similarity_distance reference :311-320 -> b2t_structure_distance
+  local_relation_fuse_motion   reference :284-310 -> the two above, fused in NumPy in the reference's operation order
+Appearance costs (cosine / euclidean GEMMs, out of the section-8 hot path) run on the GPU through torch.
 """
 import numpy as np
 
@@ -170,12 +172,36 @@ def matching_cascade(distance_metric, matching_thresh, cascade_depth, tracks, de
     return matches, unmatched_tracks, todo
 
 
-def _uavmot_unavailable(*a, **k):
-    raise NotImplementedError("UAVMOT structure costs (reference matching.py:284-389) are outside the accelerated "
-                              "detect->NMS->associate path (SURVEY.md section 2.1 row 3) and are not provided")
+def structure_representation(tracks, mode='trcak'):
+    """(n, 3) float64 [max, min, angle] per track (SURVEY q22): mode 'detection' takes get_xy() (float32), any other mode the
+    Kalman centre mean[0:2] (float64).  An empty list gives an empty (0,) array, as the reference's np.asarray([])."""
+    if len(tracks) == 0:
+        return np.asarray([])
+    ops = _eng.ops()
+    if mode == "detection":
+        pts = ops.dev(np.array([np.asarray(t.get_xy(), np.float32)[:2] for t in tracks], np.float32), torch.float32)
+    else:
+        pts = ops.dev(np.array([np.asarray(t.mean, np.float64)[:2] for t in tracks], np.float64), torch.float64)
+    return ops.structure_vectors(pts, detection=mode == "detection").cpu().numpy()
 
 
-local_relation_fuse_motion = structure_similarity_distance = structure_representation = _uavmot_unavailable
+def structure_similarity_distance(tracks, detections):
+    """max(0, cdist(track structure, detection structure, 'cosine')); (n, m) zeros when either list is empty (the reference's cdist
+    raises on the empty (0,) arrays there)."""
+    if len(tracks) == 0 or len(detections) == 0:
+        return np.zeros((len(tracks), len(detections)), dtype=np.float64)
+    ops = _eng.ops()
+    a = ops.dev(structure_representation(tracks), torch.float64)
+    b = ops.dev(structure_representation(detections, mode='detection'), torch.float64)
+    return ops.structure_distance(a, b).cpu().numpy()
+
+
+def local_relation_fuse_motion(cost_matrix, tracks, detections, only_position=False, lambda_=0.98):
+    """lambda_ * cost_matrix + (1 - lambda_) * structure distance (UAVMOT's association 1)"""
+    if cost_matrix.size == 0:
+        return cost_matrix
+    structure_distance = structure_similarity_distance(tracks, detections)
+    return lambda_ * cost_matrix + (1 - lambda_) * structure_distance
 
 
 def angle(v1, v2):
