@@ -218,7 +218,7 @@ typedef struct b2t_conv_desc {
     int act;              /* 1 = SiLU, 0 = linear, 2 = ReLU (the ReID extractor, tracker/reid_models/deepsort_reid.py), 3 = LeakyReLU(0.1) (YOLOv7-tiny) */
     int out_f32;          /* 1 = fp32 output, 0 = bf16 */
     int block_n;          /* 0 = automatic; else output channels per CTA (multiple of 16, <= 256; rounded up to 32, 64, 128 or 256) */
-    int tile_w;           /* 0 = automatic; else spatial tile width (4, 8 or 16) */
+    int tile_w;           /* 0 = automatic; else spatial tile width (4, 8 or 16), or 128 = runs of 128 pixels of the flattened output (3x3) */
     int stages;           /* 0 = automatic (as deep as shared memory allows); else shared-memory ring depth (1..8) */
     int in_row_pixels;    /* 0 = w; else pixels per input row in memory (rows padded on the right; x points at column 0) */
     int rowpack;          /* 1 = "row-packed" 3x3 / stride 1 / cin 16 layer (the w6 stem after ReOrg): the three kw taps of a

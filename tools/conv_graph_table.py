@@ -3,7 +3,8 @@ every launch, its time alone (back-to-back CUDA-event timing, the autotuner's ow
 (difference between the CUDA graphs of ops[0..k] and ops[0..k-1], programmatic dependent launch overlap included), next to the
 layer's floors: flops / sustained tensor peak and algorithmic bytes / HBM peak (MEASURED_PEAKS.json, else the H100 SXM data sheet:
 989 TFLOP/s dense fp16, 3 350 GB/s -- a power-capped card reaches less, so the floors are optimistic there).  'pp' / 'co' = consumer
-schedule: ping-pong (one warpgroup's epilogue under the other's MMAs) or cooperative.
+schedule: ping-pong (one warpgroup's epilogue under the other's MMAs) or cooperative; 'run' / 'pat' = the 128 pixels of a sub-tile
+are a run of the flattened output axis (tile_w = 128, im2col boxes) or a spatial patch (3x3 layers; 1x1 layers are always runs).
 
     python tools/conv_graph_table.py [out.txt]
 """
@@ -64,9 +65,10 @@ def main(out_path=None, batch=8, size=1280):
         by = g["n"] * (g["h"] * g["w"] * cin * 2 + ho * wo * g["cout"] * (4 if g["out_f32"] else 2)) + g["k"] * g["k"] * cin * g["cout"] * 2
         tf, th = fl / peak * 1e6, by / hbm * 1e6
         floor, alone = max(tf, th), t.get("us", float("nan"))
-        cfg = "%4d>%4d k%d s%d %3dx%-3d bn%3d mt%d %s st%d v%d g%3d" % (g["cin"], g["cout"], g["k"], g["stride"], g["h"], g["w"], inf["bn"], inf["mt"],
-                                                             "pp" if inf["pingpong"] else "co", inf["stages"], t.get("variant", 0), inf["grid"])
-        out.append("%-24s %-51s alone %6.1f  in-graph %6.1f us %6.0f TFLOP/s  floor %6.1f (%s) x%4.1f" %
+        px = "run" if g["k"] == 1 or t.get("tile_w") == 128 else "pat"
+        cfg = "%4d>%4d k%d s%d %3dx%-3d bn%3d mt%d %s %s st%d v%d g%3d" % (g["cin"], g["cout"], g["k"], g["stride"], g["h"], g["w"], inf["bn"], inf["mt"],
+                                                                "pp" if inf["pingpong"] else "co", px, inf["stages"], t.get("variant", 0), inf["grid"])
+        out.append("%-24s %-55s alone %6.1f  in-graph %6.1f us %6.0f TFLOP/s  floor %6.1f (%s) x%4.1f" %
                    (name.replace("model.", "L").replace(".conv", ""), cfg, alone, d_us, fl / max(d_us, 1e-3) / 1e6, floor, "tensor" if tf >= th else "hbm", d_us / floor))
         tot_in += d_us; tot_alone += alone; tot_floor += floor
         if d_us / floor > worst[0]:

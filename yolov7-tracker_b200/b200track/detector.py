@@ -27,30 +27,52 @@ def _check(lib, rc, what):
 _TUNE_CACHE = {}      # layer signature -> (variant index, tile configuration, record): see DetectorW6._tuned_plan
 
 
-def conv_variants(w, k, s, cin, dtype, stem_row=None):
+class ConvVariants(list):
+    """What ``conv_variants`` returns: the list of variants, plus ``out_geom`` = (n, ho, wo), the output map of the launch (None
+    when it reads the padded stem buffer), from which ``conv_candidates`` decides whether pixel runs are worth timing."""
+    def __init__(self, items, out_geom=None):
+        super().__init__(items)
+        self.out_geom = out_geom
+
+
+def conv_variants(w, k, s, cin, dtype, stem_row=None, out_geom=None):
     """The addressing variants of one conv launch: [(packed weights, extra ConvPlan arguments)], the default first.  w: the fp32
-    (Cout, Cin, k, k) weight, Cin already padded; stem_row: the row pitch in pixels when the conv reads the padded ReOrg stem buffer."""
+    (Cout, Cin, k, k) weight, Cin already padded; stem_row: the row pitch in pixels when the conv reads the padded ReOrg stem buffer;
+    out_geom: (n, ho, wo) of the output map."""
     if stem_row is not None:        # the stem reads the padded ReOrg buffer: row-packed first, generic addressing as the fallback
-        return [(pack_conv_weight_rowpack(w, dtype=dtype), dict(rowpack=True, in_row_pixels=stem_row, x_pixel0=0)),
-                (pack_conv_weight(w, dtype=dtype), dict(in_row_pixels=stem_row, x_pixel0=1)),
-                (pack_conv_weight(w, dtype=dtype), dict(in_row_pixels=stem_row, x_pixel0=1, halo=1))]
-    variants = [(pack_conv_weight(w, dtype=dtype), {})]
+        return ConvVariants([(pack_conv_weight_rowpack(w, dtype=dtype), dict(rowpack=True, in_row_pixels=stem_row, x_pixel0=0)),
+                             (pack_conv_weight(w, dtype=dtype), dict(in_row_pixels=stem_row, x_pixel0=1)),
+                             (pack_conv_weight(w, dtype=dtype), dict(in_row_pixels=stem_row, x_pixel0=1, halo=1))])
+    variants = ConvVariants([(pack_conv_weight(w, dtype=dtype), {})], out_geom)
     if k == 3 and s == 1 and cin % 64 == 0:         # halo-tile addressing competes with one-tile-per-tap
         variants.append((variants[0][0], dict(halo=1)))
     return variants
+
+
+def pixel_runs_pay(k, out_geom):
+    """True when a 3x3 layer's best spatial patch (TH x TW = 128 pixels, TW 4, 8 or 16) computes more pixel slots than runs of 128
+    pixels of the flattened N*Ho*Wo axis (tile_w = 128) -- the 20 x 20 and 40 x 40 maps of w6 -- so exactly divisible maps pay
+    no extra tuning time."""
+    if k != 3 or out_geom is None:
+        return False
+    n, ho, wo = out_geom
+    patch = min(-(-ho // (128 // tw)) * -(-wo // tw) for tw in (4, 8, 16)) * 128 * n
+    return patch > -(-n * ho * wo // 128) * 128
 
 
 def conv_candidates(k, s, cin, cout, f32, variants):
     """Every (variant index, tile configuration) the autotuner times for one conv launch, in timing order: tile width BLOCK_N, one or
     two 128-pixel sub-tiles per tile (mt), ring depth (0 = as deep as shared memory allows, 2 / 3 = shallow rings) and, for 1x1 layers
     with whole 128-channel pairs, one or two K chunks per ring stage (kpair), for each addressing variant.  BLOCK_N 32 is offered to
-    layers of at most 32 channels only, where it is the kernel's default tiling.  Some are refused by ``b2t_conv_plan_create`` for a
-    given layer (B2TError); the autotuner skips those."""
+    layers of at most 32 channels only, where it is the kernel's default tiling.  Where ``pixel_runs_pay``, variant 0 is also offered
+    as 128-pixel runs (tile_w = 128) with the same grid.  Some are refused by ``b2t_conv_plan_create`` for a given layer (B2TError);
+    the autotuner skips those."""
     cout_pad = (cout + 15) // 16 * 16
     kpairs = (1, 2) if (k == 1 and s == 1 and cin % 128 == 0) else (0,)
     shapes = [dict(block_n=bn, mt=mt, stages=st, kpair=kp) for bn in (32, 64, 128, 256) for mt in (1, 2) for st in (0, 2, 3) for kp in kpairs
               if (bn >= 64 or cout_pad <= 32) and bn <= max(64, cout_pad) and 2 * mt * bn <= 512 and not (f32 and mt == 2 and bn > 64)]
-    return [(vi, cfg) for vi in range(len(variants)) for cfg in shapes]
+    runs = [(0, dict(cfg, tile_w=128)) for cfg in shapes] if pixel_runs_pay(k, getattr(variants, "out_geom", None)) else []
+    return [(vi, cfg) for vi in range(len(variants)) for cfg in shapes] + runs
 
 
 class DetectorW6:
@@ -171,7 +193,8 @@ class DetectorW6:
             name = "+".join(names)
             assert w.shape[0] == cout
             stem = src[0] is place[0][0] and self.stem_padded
-            variants = conv_variants(w, k, s, cin, act_dtype, self.stem_row if stem else None)
+            out_geom = (self.B, (hw_in[0] + 2 * (k // 2) - k) // s + 1, (hw_in[1] + 2 * (k // 2) - k) // s + 1)
+            variants = conv_variants(w, k, s, cin, act_dtype, self.stem_row if stem else None, out_geom)
             # untuned: the first variant the kernel accepts (the stem falls back from row-packed to generic addressing)
             plan, vi, cfg = self._tuned_plan(src, variants if (self.autotune or stem) else variants[:1], b, dst, hw_in, cin, cout, k, s, act, f32)
             self.conv_specs.append(dict(name=name, op=len(self.ops), src=src[0], in_coff=src[1], dst=dst[0], out_coff=dst[1], variants=variants, bias=b,

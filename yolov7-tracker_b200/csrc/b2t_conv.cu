@@ -15,7 +15,14 @@
 //     tensor map (C, W, H, N) at coordinates (kc*BK, wo0*s+kw-p, ho0*s+kh-p, n): out-of-bounds
 //     rows/cols are zero-filled by the TMA unit (that IS the padding), stride-2 convs use the tensor
 //     map's element strides, and the box lands in shared memory as 128 rows of BK*2 bytes with the
-//     128-/64-/32-byte swizzle -- exactly the canonical K-major wgmma operand layout.  No im2col.
+//     128-/64-/32-byte swizzle -- exactly the canonical K-major wgmma operand layout.
+//   * PIXEL RUNS (3x3, tile_w = 128): the 128 pixels of a sub-tile are instead 128 consecutive pixels of the flattened N*Ho*Wo output
+//     axis, as in flat mode, so maps that no TH x TW patch divides (20 x 20, 40 x 40) compute no padding pixels.  For tap (kh,kw) and
+//     chunk kc the A operand of the whole tile is ONE im2col box (cp.async.bulk.tensor.im2col, cuTensorMapEncodeIm2col) of 128*MT
+//     pixels x BK channels: the TMA unit walks the output pixels through a bounding box of the input (corners -pad .. pad-(k-1), the
+//     conv stride as traversal stride) in W, then H, then N order -- across rows and images -- and reads each at the tap's offset
+//     (kw, kh), zero-filling outside the image.  It lands in the same 128-row swizzled layout as the tiled boxes, and the
+//     epilogue stores through flat mode's 2-D (C, N*Ho*Wo) map.
 //   * B operand: 2-D map (K, Cout), box {BK, BLOCK_N}.
 //   * warps [0, 8 MT) are the consumers, issuing wgmma.mma_async m64 x BLOCK_N x k16 with the accumulators in registers, then
 //     the epilogue from those registers: +bias -> SiLU (one tanh.approx on the SFU) -> fp16 / bf16 (or fp32) -> 128-byte-swizzled
@@ -91,7 +98,8 @@ struct ConvParams {
                                    // (-inf, 0.1) = LeakyReLU(0.1) (YOLOv7-tiny, cfg/deploy/yolov7-tiny.yaml:15)
     int out_f32;                   // 1 = fp32 output (head), 0 = 16-bit (bf16 or fp16)
     int f16;                       // 1 = operands (and 16-bit outputs) are IEEE fp16, 0 = bf16
-    int flat;                      // 1 = 1x1/s1: pixels are the flattened N*H*W axis (2-D A map), TH/TW unused
+    int flat;                      // 1 = pixels are the flattened N*Ho*Wo axis, TH/TW unused: 1x1/s1 (2-D A map) or pixel runs
+    int im2col;                    // 1 = pixel runs (flat): the A operand of a tap is one im2col box of the tile's MT*128 output pixels
     int stages;                    // shared-memory ring depth (<= kMaxStages)
     int tiles_m, tiles_n;          // tile grid; tile t -> (m = t / tiles_n, n = t % tiles_n)
     int P;                         // TMA producer warps (1..2): a thread's bulk-tensor copies are served one after the other,
@@ -137,6 +145,12 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
     asm volatile(
         "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
         ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+// im2col mode: the box is the run of output pixels that starts at bounding-box position (w, h, n), each read at (+ow, +oh)
+__device__ __forceinline__ void tma_load_im2col_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c, int w, int h, int n, uint16_t ow, uint16_t oh) {
+    asm volatile(
+        "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
+        ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c), "r"(w), "r"(h), "r"(n), "h"(ow), "h"(oh) : "memory");
 }
 __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3) {
     asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
@@ -378,6 +392,13 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
             }
             int n0, img, ho0, wo0, k0, k1; long long pix0;
             unit_coords(u, n0, img, ho0, wo0, pix0, k0, k1);
+            if (p.im2col) {             // the run's first output pixel -> its bounding-box position (the tap offsets are added per load)
+                const int hw = p.Ho * p.Wo, q = (int)pix0;
+                img = q / hw;
+                const int r = q - img * hw;
+                ho0 = r / p.Wo;
+                wo0 = r - ho0 * p.Wo;
+            }
             if (p.halo) {
                 // one (TH+2) x (MT*TW+2) x BK-channel input tile per K chunk (zero-filled outside the image = the padding),
                 // then the nine taps' weight tiles through the B ring
@@ -420,6 +441,8 @@ conv_bias_act_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
                         uint8_t* sa = ring + stage * stage_bytes;
                         if (!pre) mbar_expect_tx(&full_bar[stage], stage_tx);
                         if (p.kpair == 2) tma_load_3d(sa, &map_a, &full_bar[stage], 0, (int)pix0, 2 * kt);      // chunks 2 kt, 2 kt + 1: one {64, rows, 2} box
+                        else if (p.im2col) tma_load_im2col_4d(sa, &map_a, &full_bar[stage], kc * p.BK, wo0 * p.stride - p.pad, ho0 * p.stride - p.pad, img,
+                                                              (uint16_t)kw, (uint16_t)kh);
                         else if (p.flat) tma_load_2d(sa, &map_a, &full_bar[stage], kc * p.BK, (int)pix0);
                         else tma_load_4d(sa, &map_a, &full_bar[stage], kc * p.BK, wo0 * p.stride + kw - p.pad_w, ho0 * p.stride + kh - p.pad, img);
                         if (!pre) load_b(stage, n0, kt, 0);
@@ -702,6 +725,19 @@ EncodeTiledFn get_encode() {
     }
     return fn;
 }
+typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                   const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*, CUtensorMapInterleave,
+                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+EncodeIm2colFn get_encode_im2col() {
+    static EncodeIm2colFn fn = nullptr;
+    if (!fn) {
+        void* p = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
+            fn = reinterpret_cast<EncodeIm2colFn>(p);
+    }
+    return fn;
+}
 CUtensorMapSwizzle swizzle_for(int bk) {
     return bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (bk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
 }
@@ -785,8 +821,16 @@ extern "C" int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_
     const int row_pixels = d->in_row_pixels > 0 ? d->in_row_pixels : d->w;
     if (row_pixels < d->w) return cfail(B2T_EINVAL, "b2t_conv_plan_create: in_row_pixels < w");
     if (row_pixels != d->w && d->kh == 1 && d->stride == 1) return cfail(B2T_EINVAL, "b2t_conv_plan_create: padded rows are not supported for 1x1 layers");
+    // pixel runs (tile_w = 128): 3x3 layers reading an unpadded NHWC map; 1x1 / stride 1 layers are flat already.  Every other
+    // im2col limit holds for these geometries (4-D bounding-box corners -1 .. -1 within [-128, 127], 128 * mt <= 1024 pixels per
+    // box, traversal stride <= 8, BK * 2 bytes <= the swizzle span).
+    const bool runs = d->tile_w == 128;
+    if (runs && !(d->kh == 3 && !halo && !rowpack && row_pixels == d->w))
+        return cfail(B2T_EINVAL, "b2t_conv_plan_create: pixel runs (tile_w = 128) need a 3x3 layer without halo, row packing or padded input rows");
     EncodeTiledFn enc = get_encode();
     if (!enc) return cfail(B2T_ECUDA, "cuTensorMapEncodeTiled is not available from the driver");
+    EncodeIm2colFn enc_im2col = runs ? get_encode_im2col() : nullptr;
+    if (runs && !enc_im2col) return cfail(B2T_ECUDA, "cuTensorMapEncodeIm2col is not available from the driver");
     b2t_conv_plan* pl = new b2t_conv_plan();
     pl->kernel = nullptr; pl->bias_pad = nullptr; pl->sched = nullptr; pl->launches = 0; pl->ws = nullptr; pl->flags = nullptr; pl->out = d->y;
     ConvParams& p = pl->p;
@@ -814,7 +858,8 @@ extern "C" int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_
     p.BN = bn;
     if (MT * bn > 256) { free_plan(pl); return cfail(B2T_EINVAL, "b2t_conv_plan_create: mt x BLOCK_N > 256: the accumulators of four consumer warpgroups exceed the register file"); }
     p.out_pitch = d->out_pitch; p.out_coff = d->out_coff; p.act = d->act == 1 ? 1 : 0; p.act_floor = d->act == 2 ? 0.0f : -INFINITY; p.act_slope = d->act == 3 ? 0.1f : 1.0f; p.out_f32 = d->out_f32; p.f16 = d->io_dtype == B2T_ACT_F16 ? 1 : 0;
-    p.flat = (d->kh == 1 && d->stride == 1) ? 1 : 0;
+    p.flat = (d->kh == 1 && d->stride == 1) || runs ? 1 : 0;
+    p.im2col = runs ? 1 : 0;
     p.total_pix = (long long)p.N * p.Ho * p.Wo;
     p.halo = halo ? 1 : 0; p.halo_bytes = 0; p.halo_bufs = 0;
     if (p.flat) { p.TH = 1; p.TW = 128; p.tiles_w = p.tiles_h = 0; }
@@ -832,7 +877,7 @@ extern "C" int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_
     }
     // flat mode: two K chunks per ring stage when the layer has an even number of 64-channel chunks (bigger TMA boxes: a box
     // costs about the same whatever its size up to tens of KB, so small activation boxes alone cap the fill rate)
-    p.kpair = (p.flat && bk == 64 && (p.Cin / bk) % 2 == 0 && d->kpair != 1) ? 2 : 1;
+    p.kpair = (p.flat && !runs && bk == 64 && (p.Cin / bk) % 2 == 0 && d->kpair != 1) ? 2 : 1;
     if (d->kpair == 2 && p.kpair != 2) { free_plan(pl); return cfail(B2T_EINVAL, "b2t_conv_plan_create: kpair = 2 needs a 1x1 / stride 1 layer with an even number of 64-channel chunks"); }
     p.sub_off = halo ? p.TW * bk * 2 : kTileM * bk * 2;
     p.ksteps = halo ? p.Cin / bk : p.KH * p.KW * (p.Cin / bk) / p.kpair;
@@ -842,7 +887,15 @@ extern "C" int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_
     const CUtensorMapDataType dt16 = p.f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
     char* a_base = reinterpret_cast<char*>(const_cast<void*>(d->x)) + (size_t)d->in_coff * 2;
     CUresult r;
-    if (p.flat && p.kpair == 2) {
+    if (runs) {
+        // bounding box of the output pixels in input coordinates: corner -pad, positions -pad + s j, Ho x Wo of them per image
+        cuuint64_t dims[4] = {(cuuint64_t)p.Cin, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.N};
+        cuuint64_t strides[3] = {(cuuint64_t)d->in_pitch * 2, (cuuint64_t)d->in_pitch * 2 * p.W, (cuuint64_t)d->in_pitch * 2 * p.W * p.H};
+        const int lower[2] = {-p.pad, -p.pad}, upper[2] = {p.pad - (p.KH - 1), p.pad - (p.KW - 1)};
+        cuuint32_t es[4] = {1, (cuuint32_t)p.stride, (cuuint32_t)p.stride, 1};
+        r = enc_im2col(&pl->map_a, dt16, 4, a_base, dims, strides, lower, upper, (cuuint32_t)bk, (cuuint32_t)(kTileM * MT), es,
+                       CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    } else if (p.flat && p.kpair == 2) {
         // (channel within a chunk, pixel, chunk): lands as [chunk][pixel][64]
         cuuint64_t dims[3] = {64, (cuuint64_t)p.total_pix, (cuuint64_t)(p.Cin / 64)};
         cuuint64_t strides[2] = {(cuuint64_t)d->in_pitch * 2, 128};
@@ -868,7 +921,7 @@ extern "C" int b2t_conv_plan_create(const b2t_conv_desc* d, b2t_conv_plan** out_
         r = enc(&pl->map_a, dt16, 4, a_base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
                 CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     }
-    if (r != CUDA_SUCCESS) { free_plan(pl); return cfail(B2T_ECUDA, "cuTensorMapEncodeTiled(A) failed: " + std::to_string((int)r)); }
+    if (r != CUDA_SUCCESS) { free_plan(pl); return cfail(B2T_ECUDA, std::string(runs ? "cuTensorMapEncodeIm2col" : "cuTensorMapEncodeTiled") + "(A) failed: " + std::to_string((int)r)); }
     // halo mode: how many filter taps travel in one weight box.  A bulk-tensor copy costs about the same whatever its size up to
     // tens of KB, so a kernel row of three taps per box fills the ring faster than one tap per box.
     const int kchunks_h = p.Cin / bk;
