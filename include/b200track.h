@@ -167,6 +167,21 @@ int b2t_tracker_step_feat(b2t_tracker* t, const float* dets, const int* det_coun
  * b [batch][m][feat_dim] float32, out [batch][n][m] (matching.embedding_distance(metric='euclidean')).  The kernel B2T_STRONGSORT
  * runs before each step; |out - exact| <= gamma_{feat_dim+3} * exact with gamma_k = k u / (1 - k u), u = 2^-53. */
 int b2t_feature_distance(const float* a, int n, const float* b, int m, int feat_dim, double* out, int batch, void* stream);
+/* DeepSORT's gallery appearance cost (matching.nearest_embedding_distance, matching.py:105-127) on the tensor cores
+ * (csrc/b2t_gallery.cu).  A feature row is stored once, packed: b2t_gallery_row_halves(feat_dim) fp16 values,
+ * [hi | lo] with kpad = feat_dim rounded up to 64 each, hi + lo = 2^8 x / |x| (normalised in float64).
+ * b2t_gallery_pack packs x [n][feat_dim] float32 into packed [n][row_halves] (16-B aligned).
+ * b2t_gallery_distance: out[t][j] = min over g < counts[t] of (1 - x_g^ . x_j^) for the packed galleries
+ * gallery [n_slots][budget][row_halves] and packed detection rows dets [m][row_halves]; counts [n_slots] int32 on the device,
+ * clamped to [0, budget]; a slot with no rows gets +inf.  out [n_slots][m] float64.  A zero feature row packs to NaN (0 / 0, as
+ * the reference's normalisation), and the minimum propagates it as NumPy's does: a slot holding one, or a zero detection row, gives NaN.
+ * |out - exact| <= (216 * 2^-23 + ceil(feat_dim / 64) * 2^-24)(1 + 2^-9) + 3 * 2^-22 + 2^-32 sqrt(feat_dim) + 2^-48
+ * (2.7e-5 at feat_dim 512), where exact is the float64 value on the exactly normalised float32 rows.
+ * Memory: a gallery of budget 100 at feat_dim 512 is 100 * 2 * 512 * 2 B = 200 KB per slot, 210 MB for 1024 slots. */
+int b2t_gallery_row_halves(int feat_dim);
+int b2t_gallery_pack(const float* x, int n, int feat_dim, void* packed, void* stream);
+int b2t_gallery_distance(const void* gallery, const int* counts, int n_slots, int budget, const void* dets, int m, int feat_dim,
+                         double* out, void* stream);
 /* UAVMOT's structure representation (matching.structure_representation): out[n][3] = [max, min, included angle] over each point's
  * neighbours at a length in (0, 400), the first index on ties; [1e-4, 1e-4, 1e-4] without neighbours, [max, min, 1e-4] when max ==
  * min.  dtype B2T_F64: pts [n][2] are track centres (mean[0:2]); B2T_F32: detection centres (get_xy(), float32 lengths).  Device

@@ -85,6 +85,9 @@ SIGNATURES = {
     "b2t_tracker_step_feat": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _P, _I, _P]),
     "b2t_tracker_set_thetas": (_I, [_P, _D, _D]),
     "b2t_feature_distance": (_I, [_P, _I, _P, _I, _I, _P, _I, _P]),
+    "b2t_gallery_row_halves": (_I, [_I]),
+    "b2t_gallery_pack": (_I, [_P, _I, _I, _P, _P]),
+    "b2t_gallery_distance": (_I, [_P, _P, _I, _I, _P, _I, _I, _P, _P]),
     "b2t_structure_vectors": (_I, [_I, _P, _I, _P, _P]),
     "b2t_structure_distance": (_I, [_P, _I, _P, _I, _P, _P]),
     "b2t_tracker_read_feature": (_I, [_P, _I, _I, _P, _P]),
@@ -160,9 +163,11 @@ REID_SYMBOLS = ["b2t_reid_crops", "b2t_maxpool3x3s2", "b2t_maxpool2x2s2", "b2t_a
 # StrongSORT's OSNet extractor (csrc/b2t_osnet.cu), also compiled for the host simulator (tests/hostsim/build_sim_osnet.py)
 OSNET_SYMBOLS = [n for n in SIGNATURES if n.startswith("b2t_osnet")]
 
-# the association branch (csrc/b2t_tracker.cu); the rest are the detector's translation units
+# the association branch (csrc/b2t_tracker.cu); the rest are the detector's translation units and the tensor-core gallery kernel
+# (csrc/b2t_gallery.cu)
 TRACKER_SYMBOLS = [n for n in SIGNATURES if not n.startswith(("b2t_conv", "b2t_detect", "b2t_image", "b2t_upsample", "b2t_spp", "b2t_nms", "b2t_letterbox", "b2t_gmc_workspace", "b2t_gmc_reset", "b2t_gmc_estimate", "b2t_gmc_prepare", "b2t_ecc",
-                                                                   "b2t_reid", "b2t_maxpool", "b2t_add_relu", "b2t_avgpool", "b2t_batchnorm", "b2t_osnet"))]
+                                                                   "b2t_reid", "b2t_maxpool", "b2t_add_relu", "b2t_avgpool", "b2t_batchnorm", "b2t_osnet",
+                                                                   "b2t_gallery"))]
 
 
 def act_dtype_code(torch_dtype):

@@ -345,6 +345,33 @@ class Ops:
         L.check(self.lib, self.lib.b2t_structure_distance(_dev_ptr(a), n, _dev_ptr(b), m, _dev_ptr(out), self._s()))
         return out
 
+    def gallery_pack(self, x):
+        """x (..., feat_dim) float32 CUDA tensor -> (..., row_halves) float16: each row normalised and split as the gallery kernel
+        reads it (include/b200track.h b2t_gallery_pack)."""
+        if not (x.is_cuda and x.dtype == torch.float32 and x.dim() >= 1):
+            raise L.B2TError("gallery_pack: x must be a float32 CUDA tensor of feature rows")
+        x = x.contiguous()
+        d = x.shape[-1]
+        out = torch.empty(x.shape[:-1] + (self.lib.b2t_gallery_row_halves(d),), dtype=torch.float16, device=self.device)
+        L.check(self.lib, self.lib.b2t_gallery_pack(_dev_ptr(x), x.numel() // max(d, 1), d, _dev_ptr(out), self._s()))
+        return out
+
+    def gallery_distance(self, gallery, counts, dets, feat_dim):
+        """gallery (T, budget, row_halves) and dets (m, row_halves) packed by gallery_pack, counts (T,) int32 CUDA tensors ->
+        (T, m) float64: min over each slot's first counts[t] rows of the cosine distance (b2t_gallery_distance)."""
+        halves = self.lib.b2t_gallery_row_halves(int(feat_dim))
+        for name, x, dim in (("gallery", gallery, 3), ("dets", dets, 2)):
+            if not (x.is_cuda and x.dtype == torch.float16 and x.is_contiguous() and x.dim() == dim and x.shape[-1] == halves):
+                raise L.B2TError("gallery_distance: %s must be a contiguous float16 CUDA tensor of %d dimensions with %d columns "
+                                 "(gallery_pack rows of feat_dim %d)" % (name, dim, halves, int(feat_dim)))
+        if not (counts.is_cuda and counts.dtype == torch.int32 and counts.is_contiguous() and tuple(counts.shape) == (gallery.shape[0],)):
+            raise L.B2TError("gallery_distance: counts must be a contiguous int32 CUDA tensor with one entry per slot")
+        t, budget, m = gallery.shape[0], gallery.shape[1], dets.shape[0]
+        out = torch.empty((t, m), dtype=torch.float64, device=self.device)
+        L.check(self.lib, self.lib.b2t_gallery_distance(_dev_ptr(gallery), _dev_ptr(counts), t, budget, _dev_ptr(dets), m, int(feat_dim),
+                                                        _dev_ptr(out), self._s()))
+        return out
+
 
 _ops = None
 

@@ -28,6 +28,7 @@ UNITS = [
     ("b2t_ecc.cu", ["--fmad=false"]),
     ("b2t_reid.cu", []),
     ("b2t_osnet.cu", ["--fmad=false"]),
+    ("b2t_gallery.cu", ["--fmad=false"]),
 ]
 
 

@@ -30,6 +30,8 @@ static int check_launch(const char* what) {
     }
     return B2T_OK;
 }
+// the gallery kernels (b2t_gallery.cu) report through b2t_last_error too
+namespace b2t { void set_tracker_error(const char* m) { g_err = m; } }
 extern "C" const char* b2t_last_error(void) { return g_err.c_str(); }
 extern "C" int b2t_version(void) { return 107; }
 extern "C" long long b2t_launch_count(void) { return g_launches; }

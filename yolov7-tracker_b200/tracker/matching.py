@@ -9,7 +9,8 @@ GPU-backed (libb200track.so):
   structure_representation     reference :344-386 -> b2t_structure_vectors   (UAVMOT; the step's own device functions)
   structure_similarity_distance reference :311-320 -> b2t_structure_distance
   local_relation_fuse_motion   reference :284-310 -> the two above, fused in NumPy in the reference's operation order
-Appearance costs (cosine / euclidean GEMMs, out of the section-8 hot path) run on the GPU through torch.
+  nearest_embedding_distance   reference :105-127 -> b2t_gallery_distance   (DeepSORT; every track's gallery in one wgmma launch)
+The other appearance costs (cosine / euclidean GEMMs, out of the section-8 hot path) run on the GPU through torch.
 """
 import numpy as np
 
@@ -118,11 +119,21 @@ def embedding_distance(tracks, detections, metric='cosine'):
 
 
 def nearest_embedding_distance(tracks, detections, metric='cosine'):
+    """min over each track's stored features of the cosine distance to each detection's last feature, for all tracks in ONE
+    tensor-core launch (b2t_gallery_distance; its error bound is in include/b200track.h)."""
     cost = np.zeros((len(tracks), len(detections)))
-    det_f = np.asarray([d.features[-1] for d in detections])
+    if cost.size == 0:
+        return cost
+    ops = _eng.ops()
+    counts = [len(t.features) for t in tracks]
+    dim = len(detections[0].features[-1])
+    gal = np.zeros((len(tracks), max(max(counts), 1), dim), dtype=np.float32)      # a track without features gets +inf
     for row, track in enumerate(tracks):
-        cost[row, :] = (1. - cal_cosine_distance(np.asarray(track.features), det_f)).min(axis=0)
-    return cost
+        gal[row, :counts[row]] = np.asarray(track.features, dtype=np.float32)
+    det_f = np.asarray([d.features[-1] for d in detections], dtype=np.float32)
+    g = ops.gallery_pack(ops.dev(gal, torch.float32))
+    d = ops.gallery_pack(ops.dev(det_f, torch.float32))
+    return ops.gallery_distance(g, ops.dev(np.asarray(counts), torch.int32), d, dim).cpu().numpy()
 
 
 def ecu_iou_distance(tracks, detections, img0_shape):
