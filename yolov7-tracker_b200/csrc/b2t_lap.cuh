@@ -88,7 +88,7 @@ template <class T> struct LapWork {
     unsigned char *sc, *rdead, *cdead;
     int* scratch;   // 64 ints
     enum { TLC = 64, MAXW = 32 };   // frontier capacity of a warp's search buffer, max warps per CTA
-    template <class A> B2T_DEV void carve(A& a, int nmax, int mmax) {
+    template <class A> B2T_HD void carve(A& a, int nmax, int mmax) {
         u = a.template take<T>(nmax); v = a.template take<T>(mmax); dist = a.template take<T>(mmax);
         x = a.template take<int>(nmax); y = a.template take<int>(mmax); pred = a.template take<int>(mmax);
         tl = a.template take<int>(mmax);
@@ -96,14 +96,6 @@ template <class T> struct LapWork {
         cur = a.template take<int>(nmax > 2 * 64 ? nmax : 2 * 64); tlw = a.template take<int>(TLC * MAXW);
         sc = a.template take<unsigned char>(mmax); rdead = a.template take<unsigned char>(nmax);
         cdead = a.template take<unsigned char>(mmax); scratch = a.template take<int>(64);
-    }
-    static void size(ArenaSize& a, int nmax, int mmax) {
-        a.take<T>(nmax); a.take<T>(mmax); a.take<T>(mmax);
-        a.take<int>(nmax); a.take<int>(mmax); a.take<int>(mmax);
-        a.take<int>(mmax);
-        a.take<int>(nmax); a.take<int>(nmax); a.take<int>(nmax);
-        a.take<int>(nmax > 2 * 64 ? nmax : 2 * 64); a.take<int>(TLC * MAXW);
-        a.take<unsigned char>(mmax); a.take<unsigned char>(nmax); a.take<unsigned char>(mmax); a.take<int>(64);
     }
 };
 

@@ -31,4 +31,6 @@ inline float __fdiv_rn(float a, float b) { return a / b; }
 // Everything is force-inlined: out-of-line device functions for the big phases would move their
 // by-reference work structs to local memory under the ABI.
 #define B2T_DEVNI __device__ __forceinline__
+// shared-memory carves: run on the device over the Arena, and on the host over an ArenaSize to size the launch
+#define B2T_HD __host__ __device__ __forceinline__
 #define B2T_FULL 0xffffffffu

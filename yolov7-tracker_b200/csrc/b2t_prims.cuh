@@ -61,10 +61,15 @@ struct Arena {
         return p;
     }
 };
-// Host-side mirror of Arena::take for sizing the launch.
+// Arena over no memory, for sizing a launch: a carve run on it hands out Arena's offsets as pointers and leaves the total in off.
 struct ArenaSize {
     size_t off = 0;
-    template <class T> void take(int n) { off = (off + 15) & ~size_t(15); off += sizeof(T) * (size_t)(n > 0 ? n : 1); }
+    template <class T> B2T_HD T* take(int n) {
+        off = (off + 15) & ~size_t(15);
+        T* p = reinterpret_cast<T*>(off);
+        off += sizeof(T) * (size_t)(n > 0 ? n : 1);
+        return p;
+    }
 };
 
 // In-place exclusive scan of a[0..n) (shared memory), all threads of the CTA participate.

@@ -1,11 +1,11 @@
 // b2t_step.cuh -- the whole per-frame tracker update as ONE kernel, one CTA per video sequence.
 //
 // Replaces, for every sequence of the batch in a single launch,
-//   BaseTracker.update   tracker/basetrack.py:368-487   (kind 0, SORT)
-//   ByteTrack.update     tracker/bytetrack.py:41-204    (kind 1)
-//   BoTSORT.update       tracker/botsort.py:313-493     (kind 2, + multi_gmc :250-269)
-//   StrongSORT.update    tracker/strongsort.py:91-250   (kind 3, track_step_ss_kernel)
-//   UAVMOT.update        tracker/uavmot.py:106-279      (kind 4, track_step_uav_kernel)
+//   BaseTracker.update   tracker/basetrack.py:368-487   (kind 0, SORT)                   policy KindIou
+//   ByteTrack.update     tracker/bytetrack.py:41-204    (kind 1)                         KindIou
+//   BoTSORT.update       tracker/botsort.py:313-493     (kind 2, + multi_gmc :250-269)   KindIou, with ReID KindReid
+//   StrongSORT.update    tracker/strongsort.py:91-250   (kind 3)                         KindStrongSort
+//   UAVMOT.update        tracker/uavmot.py:106-279      (kind 4)                         KindUavmot
 // including STrack.activate / update / re_activate / multi_predict (basetrack.py:222-339) and
 // joint_stracks / sub_stracks / remove_duplicate_stracks (:540-576).  oracle/trackers.py is the
 // CPU statement of the same machine; the quirk numbers (q3..q13) refer to SURVEY.md section 8a.
@@ -21,6 +21,7 @@
 //                                                   appearance feature, and the edges of an association that get an appearance cost
 // Everything else (boxes, lists, assignment state) lives in shared memory for the frame.
 #pragma once
+#include <type_traits>
 #include "b2t_prims.cuh"
 #include "b2t_kalman.cuh"
 #include "b2t_iou.cuh"
@@ -72,7 +73,7 @@ template <class T> struct StepSmem {
     int *se_col, *se_row; T* se_cost; int esm;   // shared-memory mirror of the CSR edges (first esm entries)
     int box_bytes;             // rowbox + colbox: idle between build_csr and the next association -> second edge window (associate())
     LapWork<T> lap;
-    template <class A> B2T_DEV void carve(A& a, int cap, int dmax, int esm_) {
+    template <class A> B2T_HD void carve(A& a, int cap, int dmax, int esm_) {
         const int mx = cap > dmax ? cap : dmax;
         rowbox = a.template take<T>(4 * cap); colbox = a.template take<T>(4 * mx); detbox = a.template take<T>(4 * dmax);
         box_bytes = (int)(reinterpret_cast<unsigned char*>(colbox + 4 * mx) - reinterpret_cast<unsigned char*>(rowbox));
@@ -89,21 +90,7 @@ template <class T> struct StepSmem {
         esm = esm_;
         se_col = a.template take<int>(esm_); se_row = a.template take<int>(esm_); se_cost = a.template take<T>(esm_);
     }
-    static size_t bytes(int cap, int dmax, int esm_) {
-        ArenaSize a;
-        const int mx = cap > dmax ? cap : dmax;
-        a.take<T>(4 * cap); a.take<T>(4 * mx); a.take<T>(4 * dmax);
-        a.take<int>(dmax); a.take<int>(dmax); a.take<int>(cap);
-        a.take<int>(cap); a.take<int>(cap); a.take<int>(dmax);
-        a.take<int>(cap); a.take<int>(dmax); a.take<int>(cap);
-        a.take<int>(cap); a.take<int>(cap); a.take<int>(cap + 1); a.take<int>(cap + 1);
-        a.take<unsigned char>(cap); a.take<unsigned char>(cap); a.take<unsigned char>(cap); a.take<unsigned char>(cap);
-        a.take<int>(64);
-        a.take<int>(mx); a.take<int>(NBINS + 2); a.take<T>(8);
-        LapWork<T>::size(a, cap, mx);
-        a.take<int>(esm_); a.take<int>(esm_); a.take<T>(esm_);
-        return a.off + 16;
-    }
+    static size_t bytes(int cap, int dmax, int esm_) { ArenaSize a; StepSmem().carve(a, cap, dmax, esm_); return a.off + 16; }
     // largest shared-memory edge mirror that still fits next to everything else
     static int fit_esm(int cap, int dmax, int ecap, size_t limit) {
         const size_t base = bytes(cap, dmax, 0) + 64;
@@ -176,7 +163,6 @@ struct AppCtx {
     const int* col_det;     // [m] detection row of each column (its feature is feats[det])
     const float* feats;     // this sequence's [dmax][feat_dim] detection features
     double theta_iou, theta_emb;
-    static constexpr bool kStruct = false;
 };
 
 // UAVMOT's structure cost (matching.py:284-386, SURVEY q22).  Each point of a set (the pool's predicted centres mean[0:2] in
@@ -256,7 +242,6 @@ B2T_DEV double uav_struct_dist(const double* u, const double* v) {
 struct StructCtx {
     const double* sv_row;   // [n][3] structure vectors of the rows (the pool)
     const double* sv_col;   // [m][3] ... of the columns (the high detections)
-    static constexpr bool kStruct = true;
 };
 
 // Stage 2b of build_csr: one warp per listed edge (list[q] = edge index, top bit set when the edge lives in the global workspace
@@ -296,13 +281,11 @@ B2T_DEVNI int app_costs(const AppCtx app, const float* tfeat, int D, const int* 
     return lowered;
 }
 
-template <class X> struct NoDeduce { using type = X; };
-
 // Ctx = StructCtx: UAVMOT's fused cost replaces the IoU distance of every candidate (app is then that context, never null).
 template <class T, class Ctx = AppCtx>
 B2T_DEVNI bool build_csr(SeqView<T>& v, StepSmem<T>& sm, int n, int m, T thresh, int* dbg = nullptr, long long* dbgt = nullptr,
-                         const typename NoDeduce<Ctx>::type* app = nullptr) {
-    constexpr bool STRUCT = Ctx::kStruct;
+                         const Ctx* app = nullptr) {
+    constexpr bool STRUCT = std::is_same<Ctx, StructCtx>::value;
     const int tid = (int)threadIdx.x, nthr = (int)blockDim.x, lane = lane_id();
     int* misc = sm.misc;
     const T* colbox = sm.colbox;
@@ -553,16 +536,16 @@ template <class T> B2T_DEV LapCsr<T> step_csr(StepCtx<T>& c, int w2_base = 0, in
     return g;
 }
 
-// DENSE: the candidates are every pair whose StrongSORT cost is below thresh (build_csr_dense, *dense), not the overlapping ones.
-// Ctx = StructCtx: UAVMOT's fused cost over the overlapping pairs (build_csr's cost hook, *app).
-template <class T, bool DENSE = false, class Ctx = AppCtx>
+// Ctx = DenseCtx: the candidates are every pair whose StrongSORT cost is below thresh (build_csr_dense), not the overlapping ones.
+// Ctx = StructCtx: UAVMOT's fused cost over the overlapping pairs (build_csr's cost hook).
+template <class T, class Ctx = AppCtx>
 B2T_DEVNI void associate(StepCtx<T>& c, int n, int m, T thresh, int* err, long long* tsplit, int* dbg = nullptr,
-                         const typename NoDeduce<Ctx>::type* app = nullptr, const DenseCtx* dense = nullptr) {
+                         const Ctx* ctx = nullptr) {
     StepSmem<T>& sm = c.sm;
     long long dt = phase_clock();
     bool ok;
-    if constexpr (DENSE) ok = build_csr_dense<T>(c.v, sm, n, m, thresh, *dense);
-    else ok = build_csr<T, Ctx>(c.v, sm, n, m, thresh, dbg, &dt, app);
+    if constexpr (std::is_same<Ctx, DenseCtx>::value) ok = build_csr_dense<T>(c.v, sm, n, m, thresh, *ctx);
+    else ok = build_csr<T, Ctx>(c.v, sm, n, m, thresh, dbg, &dt, ctx);
     if (!ok && threadIdx.x == 0) *err |= ERR_EDGES;
     // The rows that did not fit the shared-memory edge mirror live in the global edge workspace.  rowbox / colbox are dead from
     // here to the next association (each one refills them): the first spilled rows are copied into that memory, so that the
@@ -689,18 +672,40 @@ B2T_DEVNI void copy_features(float* tfeat, int D, const int* slots, const int* d
 
 #define B2T_PHASE(idx) do { if (tid == 0) { const long long now_ = phase_clock(); stat[STAT_PHASE0 + (idx)] = (int)(now_ - tprev); tprev = now_; } } while (0)
 
-// APP: the BoT-SORT-with-ReID instantiation (feat_dim > 0).  The IoU-only trackers run the APP = false one, which compiles to the
-// same code as without appearance support.
-// SS (with APP): StrongSORT.update (strongsort.py:91-250).  dist_all [S][cap][dmax] holds the Euclidean distances feat_dist_kernel
-// computed for this frame (tracked and lost lists at frame start x detection rows); gamma weighs the IoU distance in the fused cost.
-// UAV (without APP): UAVMOT.update (uavmot.py:106-279).  uav_all [S][uav_seq_doubles(cap, dmax)] is the per-sequence scratch of the
-// structure vectors (uav_seq_doubles); the association-2 stage and the list algebra are StrongSORT's (q21 is q18).
-template <class T, bool APP, bool SS = false, bool UAV = false>
+// The step's policies: one type per instantiation, one member per behaviour where the kinds differ.  SORT, ByteTrack and BoT-SORT
+// share KindIou and tell each other apart at run time (p.kind).
+//   kFeat        feature state (feat_dim > 0): STrack.update's EMA (basetrack.py:323-332), a birth's copy of its detection's
+//                feature (basetrack.py:101-102), stat words 30/31.
+//   kOneSet      one detection set, score > det_thresh, no low-score set (strongsort.py:118); SORT's is a run-time test.
+//   kGmc         a camera-motion step (botsort.py:250-269, strongsort.py:140-147); of the KindIou kinds only BoT-SORT's, at run time.
+//   kWarpFirst   the pool alone is warped, BEFORE the prediction (strongsort.py:140-147); multi_gmc leaves float64 means, so the
+//                process noise is then evaluated in float64.  Otherwise pool and unconfirmed tracks are warped after it.
+//   kDense       associations 1 and 3 take build_csr_dense's fused cost (strongsort.py:150-157, :206-208).
+//   kStructSolve q20: association 1 is solved again on the structure cost (uavmot.py:184, matching.py:284-386).
+//   kQ18         q18 / q21: association 2's u_tracks1_idx index u_tracks0, but the track marked lost is strack_pool[idx]
+//                (strongsort.py:195-198, uavmot.py:228-231).  With it only association 1's Tracked leftovers go on (strongsort.py:171,
+//                uavmot.py:205), dupa records what the frame did to each pool row, the list algebra re-adds the updated tracks q18
+//                marked lost (strongsort.py:233, uavmot.py:262), and an old lost track is "not re-found" by its frame_id.
+//   kChain       (with kQ18) association 2 takes association 1's leftover high detections and updates their features, association
+//                3 association 2's leftovers (strongsort.py:174-191); else association 2 takes the low ones (uavmot.py:211-224).
+struct KindIou {                    // bytetrack.py:41-204, botsort.py:313-493, basetrack.py:368-487
+    static constexpr bool kFeat = false, kOneSet = false, kGmc = true, kWarpFirst = false, kDense = false, kStructSolve = false,
+                          kQ18 = false, kChain = false;
+};
+struct KindReid : KindIou { static constexpr bool kFeat = true; };     // BoT-SORT with ReID, botsort.py:386-392, :440-446
+struct KindStrongSort : KindIou {   // strongsort.py:91-250
+    static constexpr bool kFeat = true, kOneSet = true, kWarpFirst = true, kDense = true, kQ18 = true, kChain = true;
+};
+struct KindUavmot : KindIou { static constexpr bool kGmc = false, kStructSolve = true, kQ18 = true; };     // uavmot.py:106-279
+
+// K: one of the policies above.  dist_all [S][cap][dmax] (kDense) holds the Euclidean distances feat_dist_kernel computed for this
+// frame (tracked and lost lists at frame start x detection rows); gamma (kDense) weighs the IoU distance in the fused cost.
+// uav_all [S][uav_seq_doubles(cap, dmax)] (kStructSolve) is the per-sequence scratch of the structure vectors.
+template <class T, class K>
 B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq, const float* dets_all,
                             const int* det_count, const float* feats_all, const double* warps, const int* id_base, double* out_all,
-                            int out_rows, int* stat_all, unsigned char* smem_raw, const double* dist_all = nullptr,
-                            double gamma = 0.0, double* uav_all = nullptr) {
-    constexpr bool Q18 = SS || UAV;     // u_tracks1_idx indexes u_tracks0 but marks strack_pool[idx] lost (strongsort.py:195, uavmot.py:228)
+                            int out_rows, int* stat_all, unsigned char* smem_raw, const double* dist_all, double gamma,
+                            double* uav_all) {
     StepCtx<T> c(st, seq, prm);
     Arena arena(smem_raw);
     c.sm.carve(arena, st.cap, st.dmax, st.esm);
@@ -715,10 +720,10 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
     int* err = &sm.misc[48];
     long long tprev = phase_clock();
     // detection features [dmax][feat_dim] of this sequence (BoT-SORT with ReID), null otherwise
-    const float* feats = APP && feats_all && !p.predict_only ? feats_all + (size_t)seq * st.dmax * st.feat_dim : nullptr;
+    const float* feats = K::kFeat && feats_all && !p.predict_only ? feats_all + (size_t)seq * st.dmax * st.feat_dim : nullptr;
 
     if (tid == 0) {
-        if (APP) { sm.misc[54] = 0; sm.misc[55] = 0; }
+        if (K::kFeat) { sm.misc[54] = 0; sm.misc[55] = 0; }
         for (int q = 0; q < 48; ++q) stat[STAT_PHASE0 + q] = 0;
         *err = v.ctrl[CTRL_ERR];
         if (id_base) v.ctrl[CTRL_NEXT_ID] = id_base[seq];
@@ -750,7 +755,7 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         return d[3] - d[1] != 0.f && (p.fmt != FMT_XYWH || d[2] - d[0] != 0.f);
     };
     int nhi, nlo;
-    if (SS || p.kind == KIND_SORT) {      // StrongSORT: score > det_thresh, no low-score set (strongsort.py:118)
+    if (K::kOneSet || p.kind == KIND_SORT) {
         nhi = block_compact(nd, [&](int i) { return dets[6 * i + 4] > p.det_thresh && has_area(i); }, sm.hi, sm.misc);
         nlo = 0;
     } else {
@@ -780,9 +785,8 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
     B2T_PHASE(1);
     // ---- P2: Kalman predict (+ camera-motion warp) for the pool, warp for the unconfirmed
     T warp6[6];
-    // StrongSORT warps the pool only, BEFORE the prediction (strongsort.py:140-147); multi_gmc leaves float64 means, so the process
-    // noise is then evaluated in float64
-    const bool gmc = p.use_gmc && (SS || p.kind == KIND_BOTSORT) && warps != nullptr && !p.predict_only;
+    // (StrongSORT, the kind that warps first, always has the step; of the KindIou kinds only BoT-SORT)
+    const bool gmc = K::kGmc && p.use_gmc && (K::kWarpFirst || p.kind == KIND_BOTSORT) && warps != nullptr && !p.predict_only;
     if (gmc) for (int q = 0; q < 6; ++q) warp6[q] = (T)warps[(size_t)seq * 6 + q];
     {
         const int r = lane_id() & 7, grp = lane_id() >> 3;
@@ -793,15 +797,15 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
             KRow<T> kr;
             if (on) kf_load<T>(kr, v.mean + (size_t)slot * 8, v.cov + (size_t)slot * 64, r);
             else { kr.m = (T)0; for (int j = 0; j < 8; ++j) kr.p[j] = (T)0; }
-            if constexpr (SS) { if (gmc) kf_gmc<T>(kr, r, warp6); }
-            kf_predict<T>(kr, r, p.fmt, on && sm.pstate[k] != ST_TRACKED, (SS && gmc) ? false : q_f32);
-            if (!SS && gmc) kf_gmc<T>(kr, r, warp6);
+            if constexpr (K::kWarpFirst) { if (gmc) kf_gmc<T>(kr, r, warp6); }
+            kf_predict<T>(kr, r, p.fmt, on && sm.pstate[k] != ST_TRACKED, (K::kWarpFirst && gmc) ? false : q_f32);
+            if (!K::kWarpFirst && gmc) kf_gmc<T>(kr, r, warp6);
             if (on) {
                 kf_store<T>(kr, v.mean + (size_t)slot * 8, v.cov + (size_t)slot * 64, r);
                 if (r == 0) v.flags[slot] &= ~1;
             }
         }
-        if (!SS && gmc) {
+        if (!K::kWarpFirst && gmc) {
             for (int base = warp_id() * 4; base < nunc; base += num_warps() * 4) {
                 const int k = base + grp;
                 const bool on = k < nunc;
@@ -830,18 +834,17 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         B2T_PHASE(3);
         long long tsplit = tprev;
         const AppCtx app1 = {sm.pool, sm.hi, feats, p.theta_iou, p.theta_emb};
-        // StrongSORT: per pool row, what this frame did to it (read by the list algebra, P9): 1 updated in association 1,
+        const double* dist = K::kDense ? dist_all + (size_t)seq * cap * st.dmax : nullptr;
+        // kQ18: per pool row, what this frame did to it (read by the list algebra, P9): 1 updated in association 1,
         // 2 re-activated in association 1, 4 updated in association 2, 8 marked lost by q18
-        const double* dist = SS ? dist_all + (size_t)seq * cap * st.dmax : nullptr;
-        if constexpr (SS) {
-            for (int k = tid; k < npool; k += nthr) sm.dupa[k] = 0;
+        if constexpr (K::kQ18) for (int k = tid; k < npool; k += nthr) sm.dupa[k] = 0;
+        if constexpr (K::kDense) {
             const DenseCtx d1 = {sm.pool, sm.hi, dist, st.dmax, gamma};
-            associate<T, true>(c, npool, nhi, (T)p.t1, err, &tsplit, stat + STAT_SUB0, nullptr, &d1);
+            associate<T, DenseCtx>(c, npool, nhi, (T)p.t1, err, &tsplit, stat + STAT_SUB0, &d1);
         } else {
-            if constexpr (UAV) for (int k = tid; k < npool; k += nthr) sm.dupa[k] = 0;
             associate<T>(c, npool, nhi, (T)p.t1, err, &tsplit, stat + STAT_SUB0, feats ? &app1 : nullptr);
         }
-        if constexpr (UAV) {
+        if constexpr (K::kStructSolve) {
             // q20 (uavmot.py:184): the IoU solve at 0.7 only decides whether the fused solve runs -- it does when matched_pair0.any(),
             // i.e. some match other than the single pair (0, 0); the fused solve at 0.8 then replaces its result
             const int* x0 = sm.lap.x;
@@ -871,7 +874,7 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
                 __syncthreads();
                 const StructCtx sc = {sv_t, sv_d};
                 // its CSR / LAP boundary ends phase 4 and its LAP is phase 5: the two solves and the structure scans are all counted
-                associate<T, false, StructCtx>(c, npool, nhi, (T)UAV_T1, err, &tsplit, stat + STAT_SUB0, &sc);
+                associate<T, StructCtx>(c, npool, nhi, (T)UAV_T1, err, &tsplit, stat + STAT_SUB0, &sc);
             }
         }
         if (tid == 0) { stat[STAT_PHASE0 + 4] = (int)(tsplit - tprev); tprev = tsplit;
@@ -889,7 +892,7 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         int nut;
         if (sort)
             nut = block_compact(npool, [&](int i) { return x[i] < 0 && sm.pstate[i] == ST_TRACKED; }, sm.ut, sm.misc);
-        else if (Q18 || p.kind == KIND_BYTETRACK)    // strongsort.py:171, uavmot.py:205: only the Tracked leftovers go on
+        else if (K::kQ18 || p.kind == KIND_BYTETRACK)    // strongsort.py:171, uavmot.py:205: only the Tracked leftovers go on
             nut = block_compact(npool, [&](int i) { return x[i] < 0 && sm.pstate[i] == ST_TRACKED; }, sm.ut, sm.misc);
         else
             nut = block_compact(npool, [&](int i) { return x[i] < 0; }, sm.ut, sm.misc);
@@ -903,7 +906,7 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         apply_matches<T>(c, sm.pool, npool, dets, sm.ntr, sm.used);
         if (feats) ema_features(v.feat, v.feat_dim, sm.pool, npool, feats, sm.ntr, sm.used);
         B2T_PHASE(6);
-        if constexpr (Q18) {
+        if constexpr (K::kQ18) {
             for (int k = tid; k < npool; k += nthr)
                 if (x[k] >= 0) sm.dupa[k] = sm.pstate[k] == ST_TRACKED ? 1 : 2;
             // ---- association 2, IoU only, 0.5: u_tracks0 (Tracked leftovers) x the leftover high detections (strongsort.py:174-191)
@@ -911,19 +914,19 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
             for (int k = tid; k < nut; k += nthr) sm.nlo[k] = sm.pool[sm.ut[k]];
             __syncthreads();
             fill_track_boxes<T>(v, p.fmt, sm.nlo, nut, sm.rowbox);
-            for (int k = tid; k < (SS ? nud0 : nlo); k += nthr)
-                for (int q = 0; q < 4; ++q) sm.colbox[4 * k + q] = sm.detbox[4 * (SS ? sm.udets0 : sm.lo)[k] + q];
+            for (int k = tid; k < (K::kChain ? nud0 : nlo); k += nthr)
+                for (int q = 0; q < 4; ++q) sm.colbox[4 * k + q] = sm.detbox[4 * (K::kChain ? sm.udets0 : sm.lo)[k] + q];
             __syncthreads();
-            associate<T>(c, nut, SS ? nud0 : nlo, (T)p.t2, err, nullptr);
+            associate<T>(c, nut, K::kChain ? nud0 : nlo, (T)p.t2, err, nullptr);
             for (int k = tid; k < nut; k += nthr) {
                 const int xx = x[k];
-                sm.ntr[k] = xx >= 0 ? (SS ? sm.udets0 : sm.lo)[xx] : -1;
+                sm.ntr[k] = xx >= 0 ? (K::kChain ? sm.udets0 : sm.lo)[xx] : -1;
                 sm.used[k] = 0;
                 if (xx >= 0) sm.dupa[sm.ut[k]] |= 4;
             }
             __syncthreads();
             apply_matches<T>(c, sm.nlo, nut, dets, sm.ntr, sm.used);
-            if constexpr (SS) ema_features(v.feat, v.feat_dim, sm.nlo, nut, feats, sm.ntr, sm.used);    // every StrongSORT detection has a feature
+            if constexpr (K::kChain) ema_features(v.feat, v.feat_dim, sm.nlo, nut, feats, sm.ntr, sm.used);    // every StrongSORT detection has a feature
             // q18 / q21 (strongsort.py:195-198, uavmot.py:228-231): u_tracks1_idx indexes u_tracks0, but the track marked lost is
             // strack_pool[idx] -- possibly one updated or re-activated this frame.  The track that really went unmatched stays Tracked.
             for (int k = tid; k < nut; k += nthr)
@@ -934,7 +937,7 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
             nlostnow = block_compact(nut, [&](int k) { return x[k] < 0 && !(sm.pstate[k] == ST_LOST && sm.dupa[k] == 8); },
                                      sm.ut, sm.misc);
             for (int k = tid; k < nlostnow; k += nthr) sm.lost_now[k] = sm.pool[sm.ut[k]];
-            if constexpr (SS) {
+            if constexpr (K::kChain) {
                 // u_det1: the detections association 2 left, for association 3 (UAVMOT's association 3 takes association 1's)
                 const int nud1 = block_compact(nud0, [&](int j) { return y[j] < 0; }, sm.lo, sm.misc);
                 for (int k = tid; k < nud1; k += nthr) sm.hi[k] = sm.udets0[sm.lo[k]];
@@ -986,9 +989,9 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
             for (int q = 0; q < 4; ++q) sm.colbox[4 * k + q] = sm.detbox[4 * sm.udets0[k] + q];
         __syncthreads();
         const AppCtx app3 = {sm.unconf, sm.udets0, feats, p.theta_iou, p.theta_emb};
-        if constexpr (SS) {
+        if constexpr (K::kDense) {
             const DenseCtx d3 = {sm.unconf, sm.udets0, dist, st.dmax, gamma};
-            associate<T, true>(c, nunc, nud0, (T)p.t3, err, nullptr, nullptr, nullptr, &d3);
+            associate<T, DenseCtx>(c, nunc, nud0, (T)p.t3, err, nullptr, nullptr, &d3);
         } else {
             associate<T>(c, nunc, nud0, (T)p.t3, err, nullptr, nullptr, feats ? &app3 : nullptr);
         }
@@ -1054,7 +1057,7 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
     // ---- P9: list algebra (bytetrack.py:186-193)
     int nt1 = block_compact(n_tracked0, [&](int k) { return v.state[v.tracked[k]] == ST_TRACKED; }, sm.ut, sm.misc);
     for (int k = tid; k < nt1; k += nthr) sm.ntr[k] = v.tracked[sm.ut[k]];
-    if constexpr (Q18) {
+    if constexpr (K::kQ18) {
         // joint_stracks(tracked, activated_starcks) (strongsort.py:233, uavmot.py:262): an updated track that q18 marked lost left the filtered
         // list and comes back here, in activated_starcks order -- association 1's updates, then association 2's
         if (!p.predict_only) {
@@ -1072,7 +1075,7 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
     // old lost entries that were not re-found and whose id was not in the removed list before this frame
     // (StrongSORT, UAVMOT: "not re-found" is frame_id != f -- a re-found track that q18 marked lost is Lost again, yet on the tracked list)
     int nl1 = block_compact(n_lost0, [&](int k) { const int s = v.lost[k];
-        return (Q18 ? v.frame_id[s] != f : v.state[s] != ST_TRACKED) && !(v.removed_at[s] != 0 && v.removed_at[s] < f); }, sm.ut, sm.misc);
+        return (K::kQ18 ? v.frame_id[s] != f : v.state[s] != ST_TRACKED) && !(v.removed_at[s] != 0 && v.removed_at[s] < f); }, sm.ut, sm.misc);
     for (int k = tid; k < nl1; k += nthr) sm.nlo[k] = v.lost[sm.ut[k]];
     __syncthreads();
     const int nl_add = block_compact(nlostnow, [&](int k) { const int s = sm.lost_now[k];
@@ -1136,7 +1139,7 @@ B2T_DEV void track_step_cta(const TrackState& st, const StepParams& prm, int seq
         stat[STAT_NOUT] = nout; stat[STAT_NEXT_ID] = v.ctrl[CTRL_NEXT_ID]; stat[STAT_NTRACKED] = nt2; stat[STAT_NLOST] = nl2;
         stat[STAT_ERR] = *err; stat[STAT_FRAME] = f; stat[STAT_NPOOL] = npool; stat[STAT_NBIRTH] = nbirth;
         stat[STAT_NHI] = nhi; stat[STAT_NLO] = nlo; stat[STAT_NEDGE] = sm.misc[50]; stat[STAT_NMATCH0] = nmatch0;
-        if (APP) { stat[STAT_NAPP] = sm.misc[55]; stat[STAT_NAPPLOW] = sm.misc[54]; }
+        if (K::kFeat) { stat[STAT_NAPP] = sm.misc[55]; stat[STAT_NAPPLOW] = sm.misc[54]; }
     }
 }
 

@@ -227,36 +227,47 @@ __global__ void lap_solve_kernel(int n, int m, T thresh, const int* e_col, const
 // b2t_lap_solve_csr: one problem per CTA, in the LapCsr shapes step_csr builds.  Entries [0, s_cap) of the mirror arrays m_* are
 // copied into shared memory (the step's se_* storage) and [w2_base, w2_base + w2cap) into the second window; the window buffer is
 // longer than any window, as the step's is, and a reader that runs past w2_end finds whatever the caller put in m_* there.
+// Its shared memory: the solver's work arrays, the mirror (smax entries, the batch's largest s_cap) and the window (w2cap entries).
+template <class T> struct LapCsrSmem {
+    LapWork<T> w;
+    int *s_col, *s_row, *w2_col, *w2_row;
+    T *s_cost, *w2_cost;
+    template <class A> B2T_HD void carve(A& a, int nmax, int mmax, int smax, int w2cap) {
+        w.carve(a, nmax, mmax);
+        s_col = a.template take<int>(smax); s_row = a.template take<int>(smax); s_cost = a.template take<T>(smax);
+        w2_col = a.template take<int>(w2cap); w2_row = a.template take<int>(w2cap); w2_cost = a.template take<T>(w2cap);
+    }
+};
+
 template <class T>
 __global__ void lap_solve_csr_kernel(const b2t_lap_csr_problem* probs, const int* row_start, const int* row_cnt, const int* e_col,
                                      const T* e_cost, const int* e_row, const int* m_col, const T* m_cost, const int* m_row,
                                      int nmax, int mmax, int smax, int w2cap, int* x, int* y, int* counters) {
     B2T_DYN_SMEM(smem_raw);
     Arena arena(smem_raw);
-    LapWork<T> w;
-    w.carve(arena, nmax, mmax);
-    int* s_col = arena.take<int>(smax); int* s_row = arena.take<int>(smax); T* s_cost = arena.take<T>(smax);
-    int* w2_col = arena.take<int>(w2cap); int* w2_row = arena.take<int>(w2cap); T* w2_cost = arena.take<T>(w2cap);
+    LapCsrSmem<T> sm;
+    sm.carve(arena, nmax, mmax, smax, w2cap);
+    LapWork<T>& w = sm.w;
     const b2t_lap_csr_problem p = probs[blockIdx.x];
     const int tid = (int)threadIdx.x, nthr = (int)blockDim.x;
     const size_t eo = (size_t)p.entry_off;
     // (the row indices are read only by the edge-parallel passes: a row-parallel problem may come without them)
     const bool rows = !p.rowwise;
-    for (int e = tid; e < p.s_cap; e += nthr) { s_col[e] = m_col[eo + e]; s_row[e] = rows ? m_row[eo + e] : -1; s_cost[e] = m_cost[eo + e]; }
+    for (int e = tid; e < p.s_cap; e += nthr) { sm.s_col[e] = m_col[eo + e]; sm.s_row[e] = rows ? m_row[eo + e] : -1; sm.s_cost[e] = m_cost[eo + e]; }
     const bool win = p.w2_end > p.w2_base;
     if (win)
         for (int k = tid; k < w2cap; k += nthr) {
             const int e = p.w2_base + k;
             const bool in = e < p.n_entries;
-            w2_col[k] = in ? m_col[eo + e] : -1; w2_row[k] = in && rows ? m_row[eo + e] : -1; w2_cost[k] = in ? m_cost[eo + e] : (T)0;
+            sm.w2_col[k] = in ? m_col[eo + e] : -1; sm.w2_row[k] = in && rows ? m_row[eo + e] : -1; sm.w2_cost[k] = in ? m_cost[eo + e] : (T)0;
         }
     __syncthreads();
     LapCsr<T> g;
     g.row_start = row_start + p.row_off; g.row_stride = 0; g.row_cnt = row_cnt + p.row_off;
     g.e_col = e_col + eo; g.e_cost = e_cost + eo;
-    g.s_col = s_col; g.s_cost = s_cost; g.s_cap = p.s_cap;
-    g.e_row = p.rowwise ? nullptr : e_row + eo; g.s_row = s_row; g.n_entries = p.rowwise ? 0 : p.n_entries;
-    if (win) { g.w2_col = w2_col; g.w2_cost = w2_cost; g.w2_row = w2_row; g.w2_base = p.w2_base; g.w2_end = p.w2_end; }
+    g.s_col = sm.s_col; g.s_cost = sm.s_cost; g.s_cap = p.s_cap;
+    g.e_row = p.rowwise ? nullptr : e_row + eo; g.s_row = sm.s_row; g.n_entries = p.rowwise ? 0 : p.n_entries;
+    if (win) { g.w2_col = sm.w2_col; g.w2_cost = sm.w2_cost; g.w2_row = sm.w2_row; g.w2_base = p.w2_base; g.w2_end = p.w2_end; }
     lap_solve_cta<T>(p.n, p.m, g, (T)p.thresh, w);
     for (int i = tid; i < p.n; i += nthr) x[(size_t)p.row_off + i] = w.x[i];
     for (int j = tid; j < p.m; j += nthr) y[(size_t)p.col_off + j] = w.y[j];
@@ -354,34 +365,16 @@ extern "C" int b2t_feature_distance(const float* a, int n, const float* b, int m
 }
 
 // ------------------------------------------------------------------------------------------ fused step
-template <class T, bool APP>
+// One parameter list for every policy K (b2t_step.cuh): a kind ignores the inputs its policy does not read (track_step_cta).
+template <class T, class K>
 __global__ void __launch_bounds__(512, 1)
 track_step_kernel(TrackState st, StepParams prm, const float* dets, const int* det_count, const float* feats, const double* warps,
-                  const int* id_base, double* out, int out_rows, int* stat) {
+                  const int* id_base, double* out, int out_rows, int* stat, const double* dist, double gamma, double* uav) {
     B2T_DYN_SMEM(smem_raw);
-    track_step_cta<T, APP>(st, prm, (int)blockIdx.x, dets, det_count, feats, warps, id_base, out, out_rows, stat, smem_raw);
+    track_step_cta<T, K>(st, prm, (int)blockIdx.x, dets, det_count, feats, warps, id_base, out, out_rows, stat, smem_raw, dist, gamma,
+                         uav);
 }
-
-// StrongSORT (B2T_STRONGSORT): its own kernel, so that the instantiations above stay as they were
-template <class T>
-__global__ void __launch_bounds__(512, 1)
-track_step_ss_kernel(TrackState st, StepParams prm, const float* dets, const int* det_count, const float* feats, const double* warps,
-                     const int* id_base, double* out, int out_rows, int* stat, const double* dist, double gamma) {
-    B2T_DYN_SMEM(smem_raw);
-    track_step_cta<T, true, true>(st, prm, (int)blockIdx.x, dets, det_count, feats, warps, id_base, out, out_rows, stat, smem_raw,
-                                  dist, gamma);
-}
-
-// UAVMOT (B2T_UAVMOT): its own kernel too, float64 only (check_cfg).  uav [S][uav_seq_doubles(cap, dmax)] is the structure-vector
-// scratch.
-template <class T>
-__global__ void __launch_bounds__(512, 1)
-track_step_uav_kernel(TrackState st, StepParams prm, const float* dets, const int* det_count, const int* id_base, double* out,
-                      int out_rows, int* stat, double* uav) {
-    B2T_DYN_SMEM(smem_raw);
-    track_step_cta<T, false, false, true>(st, prm, (int)blockIdx.x, dets, det_count, nullptr, nullptr, id_base, out, out_rows, stat,
-                                          smem_raw, nullptr, 0.0, uav);
-}
+using StepKernel = decltype(&track_step_kernel<double, KindIou>);
 
 // b2t_structure_vectors / b2t_structure_distance: the step's own device functions on caller-given sets, one CTA / one thread per pair
 template <class P>
@@ -541,7 +534,7 @@ static int lap_solve_t(const T* cost, int n, int m, int ld, double thresh, int* 
     int* e_col = (int*)p;         p += sizeof(int) * se * batch;
     int* row_cnt = (int*)p;
     ArenaSize as;
-    LapWork<T>::size(as, n, m);
+    LapWork<T>().carve(as, n, m);
     const size_t smem = as.off + 16;
     if (smem > 227 * 1024) return fail(B2T_ECAPACITY, "b2t_lap_solve: n, m too large for one CTA's shared memory");   // (nothing launched)
     const int wpb = 8;
@@ -591,9 +584,7 @@ static int lap_solve_csr_t(const b2t_lap_csr_problem* probs, int batch, const in
     }
     const int w2cap = w2max > 0 ? w2max + 64 : 0;
     ArenaSize as;
-    LapWork<T>::size(as, nmax, mmax);
-    as.take<int>(smax); as.take<int>(smax); as.take<T>(smax);
-    as.take<int>(w2cap); as.take<int>(w2cap); as.take<T>(w2cap);
+    LapCsrSmem<T>().carve(as, nmax, mmax, smax, w2cap);
     const size_t smem = as.off + 16;
     if (smem > 227 * 1024) return fail(B2T_ECAPACITY, "b2t_lap_solve_csr: n, m and the shared-memory windows need more than 227 KB per CTA");
     b2t_lap_csr_problem* d_probs = (b2t_lap_csr_problem*)align_up((size_t)ws, 256);
@@ -622,6 +613,41 @@ extern "C" int b2t_lap_solve_csr(int dtype, const b2t_lap_csr_problem* probs_hos
 }
 
 // ------------------------------------------------------------------------------------------ tracker object
+// What the host needs to know about each kind (c.kind in range: check_cfg).
+enum { FEAT_NONE, FEAT_OPTIONAL, FEAT_REQUIRED };
+struct KindFacts {
+    const char* name;
+    double t1, t2, t3;  // association thresholds: basetrack.py:414,438 (SORT), bytetrack.py:118,137,160 (ByteTrack, BoT-SORT),
+                        // strongsort.py:158,185,209, uavmot.py:182,212,235 (UAVMOT's fused solve: 0.8)
+    int feats;          // FEAT_*: appearance features (feat_dim > 0) refused, allowed or needed
+    bool f64_only;      // built for dtype B2T_F64 only: the float32 step's derived rounding bound (tests/step_bounds.py) does not
+                        // cover UAVMOT's structure cost and second solve yet
+    bool gmc;           // use_gmc is honoured (UAVMOT has no camera-motion step)
+    bool thetas;        // with features, the appearance gates theta_iou / theta_emb are read
+    bool dense;         // the dense fused cost: gamma is read, and the state block holds the frame's feature distances (dist)
+    bool structure;     // the state block holds the structure-vector scratch (uav)
+};
+static KindFacts kind_facts(const b2t_tracker_config& c) {
+    switch (c.kind) {
+    //                           name              t1                t2   t3                  feats          f64    gmc    thetas dense  structure
+    case B2T_SORT:       return {"B2T_SORT",       c.iou_thresh,     0.0, c.iou_thresh + 0.1, FEAT_NONE,     false, true,  false, false, false};
+    case B2T_BYTETRACK:  return {"B2T_BYTETRACK",  0.9,              0.5, 0.7,                FEAT_NONE,     false, true,  false, false, false};
+    case B2T_BOTSORT:    return {"B2T_BOTSORT",    0.9,              0.5, 0.7,                FEAT_OPTIONAL, false, true,  true,  false, false};
+    case B2T_STRONGSORT: return {"B2T_STRONGSORT", 0.7,              0.5, 0.7,                FEAT_REQUIRED, false, true,  false, true,  false};
+    case B2T_UAVMOT:
+    default:             return {"B2T_UAVMOT",     0.7,              0.5, 0.7,                FEAT_NONE,     true,  false, false, false, true};
+    }
+}
+
+// The step kernel of a configuration: one instantiation per policy and dtype, UAVMOT's in float64 only.
+static StepKernel step_kernel(const b2t_tracker_config& c) {
+    const bool f64 = c.dtype == B2T_F64;
+    if (c.kind == B2T_UAVMOT) return track_step_kernel<double, KindUavmot>;
+    if (c.kind == B2T_STRONGSORT) return f64 ? track_step_kernel<double, KindStrongSort> : track_step_kernel<float, KindStrongSort>;
+    if (c.feat_dim > 0) return f64 ? track_step_kernel<double, KindReid> : track_step_kernel<float, KindReid>;
+    return f64 ? track_step_kernel<double, KindIou> : track_step_kernel<float, KindIou>;
+}
+
 struct b2t_tracker {
     b2t_tracker_config cfg;
     TrackState st;
@@ -629,8 +655,8 @@ struct b2t_tracker {
     size_t smem;
     // device staging for the *_host entry point (inside the state block)
     float* d_dets; int* d_count; double* d_warps; int* d_idbase; double* d_out; int* d_stat; double* d_slot; double* d_list;
-    double* dist;   // B2T_STRONGSORT: [S][cap][dmax] feature distances of the current frame
-    double* uav;    // B2T_UAVMOT: [S][uav_seq_doubles(cap, dmax)] structure-vector scratch
+    double* dist;   // KindFacts::dense: [S][cap][dmax] feature distances of the current frame
+    double* uav;    // KindFacts::structure: [S][uav_seq_doubles(cap, dmax)] structure-vector scratch
     size_t out_rows_cap;
 };
 
@@ -663,8 +689,9 @@ static void layout(const b2t_tracker_config& c, unsigned char* base, b2t_tracker
         TAKE(st.feat, float, S * cap * (size_t)c.feat_dim);
         TAKE(st.e_app, int, S * (size_t)c.ecap);
     }
-    if (c.kind == B2T_STRONGSORT) { TAKE(dist, double, S * cap * (size_t)c.dmax); }
-    if (c.kind == B2T_UAVMOT) { TAKE(uav, double, S * uav_seq_doubles(c.cap, c.dmax)); }
+    const KindFacts k = kind_facts(c);
+    if (k.dense) { TAKE(dist, double, S * cap * (size_t)c.dmax); }
+    if (k.structure) { TAKE(uav, double, S * uav_seq_doubles(c.cap, c.dmax)); }
 #undef TAKE
     *total = align_up(L.off, 256);
 }
@@ -675,21 +702,18 @@ static int check_cfg(const b2t_tracker_config* c) {
         return fail(B2T_EINVAL, "b2t_tracker: bad kind / fmt / dtype");
     if (c->n_seq < 1 || c->cap < 64 || c->dmax < 1 || c->dmax > 1024 || c->cap > 4096 || c->ecap < 1)
         return fail(B2T_EINVAL, "b2t_tracker: bad n_seq / cap (64..4096) / dmax (1..1024) / ecap");
-    // the float32 build of the fused step has a derived rounding bound (tests/step_bounds.py) that does not cover UAVMOT's structure
-    // cost and its second solve yet: the kind runs in float64 only
-    if (c->kind == B2T_UAVMOT && c->dtype != B2T_F64)
-        return fail(B2T_EINVAL, "b2t_tracker: B2T_UAVMOT is built for dtype B2T_F64 only");
-    if (c->kind == B2T_STRONGSORT) {
-        if (c->feat_dim <= 0) return fail(B2T_EINVAL, "b2t_tracker: B2T_STRONGSORT needs appearance features (feat_dim > 0)");
-        if (!(c->gamma >= 0.0 && c->gamma <= 1.0)) return fail(B2T_EINVAL, "b2t_tracker: gamma must lie in [0, 1]");
-    }
+    const KindFacts k = kind_facts(*c);
+    if (k.f64_only && c->dtype != B2T_F64) return fail(B2T_EINVAL, "b2t_tracker: %s is built for dtype B2T_F64 only", k.name);
+    if (k.feats == FEAT_REQUIRED && c->feat_dim <= 0)
+        return fail(B2T_EINVAL, "b2t_tracker: %s needs appearance features (feat_dim > 0)", k.name);
+    if (k.dense && !(c->gamma >= 0.0 && c->gamma <= 1.0)) return fail(B2T_EINVAL, "b2t_tracker: gamma must lie in [0, 1]");
     if (c->feat_dim != 0) {
-        if (c->kind != B2T_BOTSORT && c->kind != B2T_STRONGSORT)
+        if (k.feats == FEAT_NONE)
             return fail(B2T_EINVAL, "b2t_tracker: feat_dim > 0 (appearance features) is only built for B2T_BOTSORT and B2T_STRONGSORT");
         if (c->feat_dim < 0 || c->feat_dim % 32 != 0 || c->feat_dim > 2048)
             return fail(B2T_EINVAL, "b2t_tracker: feat_dim must be 0 or a multiple of 32 up to 2048");
         // theta_iou < 1 keeps every pair with an appearance cost among the overlapping ones (the sparse candidate set)
-        if (c->kind == B2T_BOTSORT && (!(c->theta_iou < 1.0) || c->theta_emb != c->theta_emb))
+        if (k.thetas && (!(c->theta_iou < 1.0) || c->theta_emb != c->theta_emb))
             return fail(B2T_EINVAL, "b2t_tracker: theta_iou must be < 1 and theta_emb a number");
     }
     const size_t smem = c->dtype == B2T_F64 ? StepSmem<double>::bytes(c->cap, c->dmax, 0) : StepSmem<float>::bytes(c->cap, c->dmax, 0);
@@ -714,10 +738,11 @@ extern "C" int b2t_tracker_create(const b2t_tracker_config* cfg, void* state_mem
     int rc = check_cfg(cfg);
     if (rc) return rc;
     if (!state_mem || !out || ((size_t)state_mem & 255)) return fail(B2T_EINVAL, "b2t_tracker_create: state_mem must be 256-B aligned");
+    const KindFacts k = kind_facts(*cfg);
     b2t_tracker* t = new b2t_tracker();
-    // gamma is read only for B2T_STRONGSORT: a caller built against a header without it passes a shorter struct
+    // gamma is read only by the dense kinds: a caller built against a header without it passes a shorter struct
     memcpy(&t->cfg, cfg, offsetof(b2t_tracker_config, gamma));
-    t->cfg.gamma = cfg->kind == B2T_STRONGSORT ? cfg->gamma : 0.0;
+    t->cfg.gamma = k.dense ? cfg->gamma : 0.0;
     size_t total;
     layout(*cfg, (unsigned char*)state_mem, t, &total);
     t->st.n_seq = cfg->n_seq; t->st.cap = cfg->cap; t->st.dmax = cfg->dmax; t->st.ecap = cfg->ecap; t->st.feat_dim = cfg->feat_dim;
@@ -731,24 +756,13 @@ extern "C" int b2t_tracker_create(const b2t_tracker_config* cfg, void* state_mem
     p.det_thresh = (float)cfg->conf_thresh;                                                   // basetrack.py:354
     p.low_thresh = (float)((cfg->conf_thresh - 0.3) > 0.15 ? (cfg->conf_thresh - 0.3) : 0.15);  // bytetrack.py:15
     p.new_thresh = (float)(cfg->conf_thresh + 0.1);                                           // bytetrack.py:175
-    if (cfg->kind == B2T_SORT) { p.t1 = cfg->iou_thresh; p.t2 = 0.0; p.t3 = cfg->iou_thresh + 0.1; }   // basetrack.py:414,438
-    else if (cfg->kind == B2T_STRONGSORT) { p.t1 = 0.7; p.t2 = 0.5; p.t3 = 0.7; }           // strongsort.py:158,185,209
-    else if (cfg->kind == B2T_UAVMOT) { p.t1 = 0.7; p.t2 = 0.5; p.t3 = 0.7; }               // uavmot.py:182,212,235 (the fused solve: 0.8)
-    else { p.t1 = 0.9; p.t2 = 0.5; p.t3 = 0.7; }                                              // bytetrack.py:118,137,160
+    p.t1 = k.t1; p.t2 = k.t2; p.t3 = k.t3;
     p.t_dup = 0.15;                                                                           // basetrack.py:565
     p.max_time_lost = (int)(cfg->frame_rate / 30.0 * cfg->track_buffer);                      // basetrack.py:355-356
-    p.use_gmc = cfg->kind == B2T_UAVMOT ? 0 : cfg->use_gmc; p.predict_only = 0;             // UAVMOT has no camera-motion step
+    p.use_gmc = k.gmc ? cfg->use_gmc : 0; p.predict_only = 0;
     p.theta_iou = cfg->theta_iou; p.theta_emb = cfg->theta_emb;                               // botsort.py:289
     t->smem = cfg->dtype == B2T_F64 ? StepSmem<double>::bytes(cfg->cap, cfg->dmax, t->st.esm) : StepSmem<float>::bytes(cfg->cap, cfg->dmax, t->st.esm);
-    const bool app = cfg->feat_dim > 0;
-    int rs;
-    if (cfg->kind == B2T_STRONGSORT)
-        rs = cfg->dtype == B2T_F64 ? B2T_SET_SMEM((track_step_ss_kernel<double>), t->smem) : B2T_SET_SMEM((track_step_ss_kernel<float>), t->smem);
-    else if (cfg->kind == B2T_UAVMOT)
-        rs = B2T_SET_SMEM((track_step_uav_kernel<double>), t->smem);
-    else if (cfg->dtype == B2T_F64) rs = app ? B2T_SET_SMEM((track_step_kernel<double, true>), t->smem) : B2T_SET_SMEM((track_step_kernel<double, false>), t->smem);
-    else rs = app ? B2T_SET_SMEM((track_step_kernel<float, true>), t->smem) : B2T_SET_SMEM((track_step_kernel<float, false>), t->smem);
-    if (rs != 0) { delete t; return fail(B2T_ECUDA, "cannot raise dynamic shared memory"); }
+    if (B2T_SET_SMEM(step_kernel(*cfg), t->smem) != 0) { delete t; return fail(B2T_ECUDA, "cannot raise dynamic shared memory"); }
     *out = t;
     return b2t_tracker_reset(t, stream);
 }
@@ -764,32 +778,15 @@ static int step_launch(b2t_tracker* t, const float* dets, const int* det_count, 
     StepParams p = t->prm;
     p.predict_only = predict_only ? 1 : 0;
     cudaStream_t s = (cudaStream_t)stream;
-    const bool app = t->cfg.feat_dim > 0;
-    if (t->cfg.kind == B2T_STRONGSORT) {
-        const b2t_tracker_config& c = t->cfg;
-        if (!predict_only) {
-            const size_t D = (size_t)c.feat_dim;
-            const int rc = feat_dist_launch(t->st.feat, (size_t)c.cap * D, feats, (size_t)c.dmax * D, c.feat_dim, c.cap, c.dmax, t->st.ctrl,
-                                            t->st.tracked, t->st.lost, c.cap, det_count, t->dist, (size_t)c.cap * c.dmax, c.dmax, c.n_seq, s);
-            if (rc) return rc;
-        }
-        if (c.dtype == B2T_F64) {
-            auto k = track_step_ss_kernel<double>;
-            B2T_LAUNCH(k, c.n_seq, 512, t->smem, s, t->st, p, dets, det_count, feats, warps, id_base, out, out_rows, stat, t->dist, c.gamma);
-        } else {
-            auto k = track_step_ss_kernel<float>;
-            B2T_LAUNCH(k, c.n_seq, 512, t->smem, s, t->st, p, dets, det_count, feats, warps, id_base, out, out_rows, stat, t->dist, c.gamma);
-        }
-    } else if (t->cfg.kind == B2T_UAVMOT) {
-        auto k = track_step_uav_kernel<double>;
-        B2T_LAUNCH(k, t->cfg.n_seq, 512, t->smem, s, t->st, p, dets, det_count, id_base, out, out_rows, stat, t->uav);
-    } else if (t->cfg.dtype == B2T_F64) {
-        auto k = app ? track_step_kernel<double, true> : track_step_kernel<double, false>;
-        B2T_LAUNCH(k, t->cfg.n_seq, 512, t->smem, s, t->st, p, dets, det_count, feats, warps, id_base, out, out_rows, stat);
-    } else {
-        auto k = app ? track_step_kernel<float, true> : track_step_kernel<float, false>;
-        B2T_LAUNCH(k, t->cfg.n_seq, 512, t->smem, s, t->st, p, dets, det_count, feats, warps, id_base, out, out_rows, stat);
+    const b2t_tracker_config& c = t->cfg;
+    if (kind_facts(c).dense && !predict_only) {
+        const size_t D = (size_t)c.feat_dim;
+        const int rc = feat_dist_launch(t->st.feat, (size_t)c.cap * D, feats, (size_t)c.dmax * D, c.feat_dim, c.cap, c.dmax, t->st.ctrl,
+                                        t->st.tracked, t->st.lost, c.cap, det_count, t->dist, (size_t)c.cap * c.dmax, c.dmax, c.n_seq, s);
+        if (rc) return rc;
     }
+    const StepKernel k = step_kernel(c);
+    B2T_LAUNCH(k, c.n_seq, 512, t->smem, s, t->st, p, dets, det_count, feats, warps, id_base, out, out_rows, stat, t->dist, c.gamma, t->uav);
     return check_launch("track_step");
 }
 
