@@ -77,9 +77,14 @@ def ema_ref(old, f):
     return s.div(nsb)
 
 
-def check_stream(trk, frames, warps, kind, fmt, f32, stats, where="", feats=None, conf_thresh=0.2):
+def check_stream(trk, frames, warps, kind, fmt, f32, stats, where="", feats=None, conf_thresh=0.2, on_frame=None, nearest=NEAREST):
     """Runs the whole stream through trk, checking every frame.  stats gets the largest err / bound per path; returns the number of
-    slot transitions checked per path."""
+    slot transitions checked per path.  nearest: detections tried per slot (more in crowds).  A slot that leaves both lists this frame (remove_duplicate_stracks, a removed unconfirmed
+    track, long-lost pruning) is read by its slot and checked like the others: its record stays until a later frame reuses it.
+    on_frame (optional) is called after each frame's checks with a dict of what the association certificate
+    (tests/assoc_bounds.py) needs: the frame's index, tag, detections and features, the before-state ('before', in list order), the
+    checked slots ('exist'), their predicted or warped state with its bound ('base'), the float32-mean flag the association read
+    ('uflag'), the detection each slot was updated with ('matched_det', -1 for none) and trk.stat when the tracker has it."""
     dt = np.float32 if f32 else np.float64
     ss = kind == "strongsort"
     counts = dict(predict=0, update=0, birth=0, unconfirmed=0, feature=0)
@@ -91,6 +96,13 @@ def check_stream(trk, frames, warps, kind, fmt, f32, stats, where="", feats=None
         w = None if warps is None else np.asarray(warps[i], np.float64).reshape(-1)
         res = trk.step(f, fe, w)
         after = _snapshot(trk, fe is not None)
+        seen = dict(after)
+        for s in before:
+            if s not in after:                                        # left both lists: the slot's record is still this frame's
+                m, c = trk.read_slot(s)
+                seen[s] = dict(tid=before[s]["tid"], state=-1, pool=before[s]["pool"], mean=m, cov=c)
+                if fe is not None:
+                    seen[s]["feat"] = trk.read_feature(s)
         dets = np.asarray(f, np.float32).reshape(-1, 6)
         Z = R.det_to_meas(fmt, dets[:, :4]) if len(dets) else np.zeros((0, 4), np.float32)
         pool = [s for s, d in before.items() if d["pool"]]
@@ -99,14 +111,14 @@ def check_stream(trk, frames, warps, kind, fmt, f32, stats, where="", feats=None
         wk = None if w is None else w.astype(dt)
         new_flag = {}
 
-        exist = [s for s, d in after.items() if s in before and before[s]["tid"] == d["tid"]]
+        exist = [s for s, d in seen.items() if s in before and before[s]["tid"] == d["tid"]]
         born = [s for s in after if s not in exist]
         if exist:
             E = np.array(exist)
             m0 = np.stack([before[s]["mean"] for s in exist]).astype(dt)
             c0 = np.stack([before[s]["cov"] for s in exist]).astype(dt)
-            gm = np.stack([after[s]["mean"] for s in exist])
-            gc = np.stack([after[s]["cov"] for s in exist])
+            gm = np.stack([seen[s]["mean"] for s in exist])
+            gc = np.stack([seen[s]["cov"] for s in exist])
             ispool = np.array([before[s]["pool"] for s in exist])
             tracked0 = np.array([before[s]["state"] == ST_TRACKED for s in exist])
             x0 = R.state(m0, c0, f32)
@@ -127,7 +139,7 @@ def check_stream(trk, frames, warps, kind, fmt, f32, stats, where="", feats=None
             w_upd = np.full(len(exist), np.inf)
             if len(dets):
                 d2 = ((Z[None, :, :2].astype(np.float64) - gm[:, None, :2]) ** 2).sum(-1)
-                near = np.argsort(d2, axis=1)[:, :NEAREST]
+                near = np.argsort(d2, axis=1)[:, :nearest]
                 pi = np.repeat(np.arange(len(exist)), near.shape[1])
                 pj = near.reshape(-1)
                 bp = _take(base, pi)
@@ -143,14 +155,14 @@ def check_stream(trk, frames, warps, kind, fmt, f32, stats, where="", feats=None
                 np.minimum.at(w_upd, pi, wp)
             for k, s in enumerate(exist):
                 assert ok_none[k] or nmatch[k] >= 1, "%s: slot %d (id %d) is on no path of its kind (predict only %.3g, best update %.3g)" % (
-                    tag, s, after[s]["tid"], w_none[k], w_upd[k])
+                    tag, s, seen[s]["tid"], w_none[k], w_upd[k])
                 assert nmatch[k] <= 1 and not (ok_none[k] and nmatch[k]), "%s: slot %d matches more than one path" % (tag, s)
                 path = "update" if nmatch[k] else ("predict" if ispool[k] else "unconfirmed")
                 counts[path] += 1
                 stats[path] = max(stats.get(path, 0.0), float(w_upd[k] if nmatch[k] else w_none[k]))
                 new_flag[s] = False if (nmatch[k] or ispool[k] or (gmc_on and not ss)) else flag.get(s, False)
                 if fe is not None:
-                    old, got = before[s]["feat"], after[s]["feat"]
+                    old, got = before[s]["feat"], seen[s]["feat"]
                     # BoT-SORT's low-score detections carry no feature (its association 2); every StrongSORT detection has one
                     has_feat = ss or (nmatch[k] and dets[matched_det[k], 4] >= np.float32(conf_thresh))
                     if nmatch[k] and tracked0[k] and has_feat:
@@ -170,6 +182,10 @@ def check_stream(trk, frames, warps, kind, fmt, f32, stats, where="", feats=None
                 if fe is not None:
                     assert np.array_equal(after[s]["feat"], fe[int(np.argmax(okb))]), "%s: new slot %d feature" % (tag, s)
         flag = new_flag
+        if on_frame is not None:
+            on_frame(dict(i=i, tag=tag, dets=dets, feats=fe, before=before, exist=exist, base=base if exist else None,
+                          uflag=uflag if exist else None, matched_det=matched_det if exist else None,
+                          stat=np.asarray(trk.stat).reshape(-1).copy() if hasattr(trk, "stat") else None))
         # output rows
         if len(res):
             slots = res[:, 7].astype(int)
@@ -197,7 +213,8 @@ def edge_stream(seed=21, n_frames=60, n_obj=40):
 
 def case(name):
     """(kind, fmt, frames, feats, warps, tracker kwargs) of one step case: a lifecycle_golden configuration, the edge stream
-    ('edge_<kind>'), or a stream with appearance features ('feat_<kind>': StrongSORT, BoT-SORT with ReID)."""
+    ('edge_<kind>'), a stream with appearance features ('feat_<kind>': StrongSORT, BoT-SORT with ReID), or UAVMOT on a lifecycle
+    stream ('uavmot', default format)."""
     import lifecycle_golden as LG
     if name.startswith("edge_"):
         kind = name[5:]
@@ -207,6 +224,9 @@ def case(name):
         kind = name[5:]
         frames, feats, warps = make_strongsort_stream(17, 40, 40, 64)
         return kind, "strongsort" if kind == "strongsort" else "botsort", frames, feats, warps, dict(track_buffer=30, feat_dim=64)
+    if name == "uavmot":
+        frames, _ = lifecycle_stream(5, 60, 40)
+        return "uavmot", "default", frames, None, None, dict(track_buffer=30)
     cfg = LG.Config(name)
     frames, warps = cfg.stream()
     return cfg.kind, cfg.fmt, frames, None, warps, dict(track_buffer=cfg.track_buffer, frame_rate=cfg.frame_rate,
@@ -216,4 +236,4 @@ def case(name):
 def step_cases():
     import lifecycle_golden as LG
     names = LG.configs() + ["edge_bytetrack", "edge_botsort", "feat_strongsort", "feat_botsort"]
-    return [(c, d) for c in names for d in ("f32", "f64")]
+    return [(c, d) for c in names for d in ("f32", "f64")] + [("uavmot", "f64")]      # UAVMOT is built in float64 only

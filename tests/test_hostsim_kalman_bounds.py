@@ -140,7 +140,7 @@ class SimStep:
     def __init__(self, lib, kind, fmt, dtype, feat_dim=0, **kw):
         self.lib = lib
         self.cfg = L.TrackerConfig(kind=L.KIND_BY_NAME[kind], dtype=dtype, fmt=L.FMT_BY_NAME[fmt], n_seq=1, cap=kw.get("cap", 256),
-                                   dmax=kw.get("dmax", 256), ecap=8192, use_gmc=1, track_buffer=kw.get("track_buffer", 30),
+                                   dmax=kw.get("dmax", 256), ecap=kw.get("ecap", 8192), use_gmc=1, track_buffer=kw.get("track_buffer", 30),
                                    conf_thresh=kw.get("conf_thresh", 0.2), iou_thresh=0.5, frame_rate=kw.get("frame_rate", 30),
                                    feat_dim=feat_dim, theta_iou=0.5, theta_emb=0.25, gamma=0.1)
         nbytes = lib.b2t_tracker_state_bytes(C.byref(self.cfg))
